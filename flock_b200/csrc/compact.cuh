@@ -4,14 +4,16 @@
 //
 // A CTA processes tiles of CP_THREADS x I items.  For each tile it gets one bit per item ("survives"), ranks the
 // survivors in item order (packed SWAR scan for four-item groups, ballots otherwise), obtains the tile's global
-// output offset and hands every survivor its output position.  Two ways to get that offset:
+// output offset and hands every survivor its output position.  Three ways to get that offset:
 //
-//   single wave   (tiles <= resident CTAs; NEXMark q2's 10 M rows = 611 tiles; cooperative launch, tile = blockIdx.x):
+//   single wave   (tiles <= resident CTAs; cooperative launch, tile = blockIdx.x):
 //                 every tile needs the counts of ALL its predecessors and they all finish counting at about the same
 //                 time, so a chained look-back degenerates into everybody polling everybody (the largest share of
 //                 the kernel's stall samples).  Instead each CTA publishes one self-validating word
 //                 {launch epoch, count}, bumps ONE arrival counter, ONE thread per CTA polls that counter until all
 //                 tiles have arrived, then the CTA sums its predecessors' words with one strided read.
+//   rounds        (the vectorised filter, any number of tiles; cooperative launch): the single wave walks tiles
+//                 blockIdx.x + r * grid, publishing round r before it reads round r - 1 (cp_round_publish / _offset).
 //   many waves    persistent CTAs draw tiles from an atomic ticket; decoupled look-back with the whole CTA (thread i
 //                 inspects predecessor i): earlier waves have long published their inclusive prefixes, so one 256-wide
 //                 window almost always suffices.
@@ -210,17 +212,61 @@ __device__ __forceinline__ void cp_block_lookback(CompactSmem<E, I>& s, const Co
   __syncthreads();
 }
 
-// Ranks the survivors of one tile (bit k of `bits` = item k survives).  On return (after the internal
-// barriers) cp_position() gives every survivor its output slot and s.tile_total the tile's survivor count.
-struct CpNoHook {
-  __device__ __forceinline__ void operator()() const {}
-};
+// ---- cooperative rounds: one wave of resident CTAs, CTA b takes tiles b, b + grid, b + 2 grid, ... --------------
+// Round r is the contiguous band of tiles [r * grid, min((r + 1) * grid, num_tiles)).  A CTA publishes its tile's
+// word of round r as soon as the tile is ranked (cp_round_publish) and only then asks for the offset of its tile of
+// round r - 1 (cp_round_offset) and writes that tile: the publish of one round never waits behind the writes of the
+// previous one, so a CTA that is slow to write does not hold up everybody's next round.  With publishes one round
+// ahead, an arrival count cannot tell which round is complete, so the reader polls the epoch-tagged words themselves;
+// by the time a round is read its words were published about one tile earlier, and a stale word is rare.  The
+// arrival counter is still bumped once per tile, which keeps it in step with the host's count (launch_compact).
+__device__ __forceinline__ void cp_round_publish(const CompactScratch& sc, long long tile, unsigned long long total) {
+  if (threadIdx.x == 0) {
+    const unsigned long long tag = (unsigned long long)(sc.epoch & 0xfffffu) << 44;
+    st_relaxed_u64(sc.counts + tile, tag | EP_PREFIX | total);
+    red_relaxed_add_u32(sc.counters + 1, 1u);
+  }
+}
 
-// `before_wait` runs after the tile-local ranking and before the wait for the grid-wide prefix: work that does not
-// need output positions (prefetching the survivors' pass-through values) hides behind that wait.
-template <int E, int I, class Hook = CpNoHook>
-__device__ __forceinline__ void cp_rank_tile(CompactSmem<E, I>& s, const CompactScratch& sc, long long tile, unsigned long long bits,
-                                             unsigned (&lane_prefix)[I / E], Hook before_wait = Hook{}) {
+// Reads the words of `tile`'s round once, summing those before the tile and the whole round.  `done` (shared) holds the
+// survivors of the rounds the CTA has already read; the CTA reads its rounds in order, starting at round0 == 0.
+// On return s.excl is the tile's output offset.
+template <int E, int I>
+__device__ __forceinline__ void cp_round_offset(CompactSmem<E, I>& s, const CompactScratch& sc, long long tile, long long round0,
+                                                unsigned long long& done) {
+  // a round's survivors (at most grid x tile items) fit the 32-bit halves of the packed sum below
+  static_assert(CP_THREADS * I <= (1 << 16), "tile too large for the packed round sums");
+  const int tid = threadIdx.x;
+  const unsigned long long tag = (unsigned long long)(sc.epoch & 0xfffffu) << 44;
+  const long long round_end = round0 + sc.grid < sc.num_tiles ? round0 + sc.grid : sc.num_tiles;
+  unsigned long long part = 0;  // [31:0] words before `tile`, [63:32] all words of the round
+  for (long long i = round0 + tid; i < round_end; i += CP_THREADS) {
+    unsigned long long w = ld_relaxed_u64(sc.counts + i);
+    while ((w >> 44) != (tag >> 44)) {
+      if (sc.poll_sleep_ns) __nanosleep(sc.poll_sleep_ns);
+      w = ld_relaxed_u64(sc.counts + i);
+    }
+    const unsigned long long c = w & EP_VALUE_MASK;
+    part += (c << 32) | (i < tile ? c : 0ull);
+  }
+  const unsigned long long sums = cp_block_sum(s, part);
+  if (tid == 0) {
+    const unsigned long long before = round0 == 0 ? 0ull : done;
+    const unsigned long long excl = before + (sums & 0xffffffffull);
+    s.excl = excl;
+    done = before + (sums >> 32);
+    if (tile == sc.num_tiles - 1) {
+      *sc.out_count = excl + s.tile_total;
+      if (sc.host_count) *reinterpret_cast<volatile unsigned long long*>(sc.host_count) = excl + s.tile_total;
+    }
+  }
+  __syncthreads();
+}
+
+// Ranks the survivors of one tile within the tile (bit k of `bits` = item k survives): on return (after the internal
+// barriers) s.group_warp, lane_prefix and s.tile_total hold everything cp_local_position() needs.
+template <int E, int I>
+__device__ __forceinline__ void cp_rank_local(CompactSmem<E, I>& s, unsigned long long bits, unsigned (&lane_prefix)[I / E]) {
   constexpr int G = I / E;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   if constexpr (E == 4) {
@@ -290,6 +336,20 @@ __device__ __forceinline__ void cp_rank_tile(CompactSmem<E, I>& s, const Compact
     if (lane == 0) s.tile_total = total;
   }
   __syncthreads();
+}
+
+// Ranks the survivors of one tile (bit k of `bits` = item k survives).  On return (after the internal
+// barriers) cp_position() gives every survivor its output slot and s.tile_total the tile's survivor count.
+struct CpNoHook {
+  __device__ __forceinline__ void operator()() const {}
+};
+
+// `before_wait` runs after the tile-local ranking and before the wait for the grid-wide prefix: work that does not
+// need output positions (prefetching the survivors' pass-through values) hides behind that wait.
+template <int E, int I, class Hook = CpNoHook>
+__device__ __forceinline__ void cp_rank_tile(CompactSmem<E, I>& s, const CompactScratch& sc, long long tile, unsigned long long bits,
+                                             unsigned (&lane_prefix)[I / E], Hook before_wait = Hook{}) {
+  cp_rank_local<E, I>(s, bits, lane_prefix);
   before_wait();
   if (sc.single_wave) cp_grid_prefix(s, sc, tile, s.tile_total);
   else cp_block_lookback(s, sc, tile, s.tile_total);
@@ -297,8 +357,10 @@ __device__ __forceinline__ void cp_rank_tile(CompactSmem<E, I>& s, const Compact
 
 // Host side (core.cu): sizes the scratch and fills a CompactScratch for ONE launch over `num_tiles` tiles by a kernel of
 // which `resident_ctas` fit on the device at once; chooses the mode and the grid (sc.grid) and draws a launch epoch.
-// Call it right before launch_compact(), which advances the ticket / arrival bookkeeping once the launch is accepted.
-CompactScratch prepare_compact(const CtxPtr& ctx, long long num_tiles, long long resident_ctas, unsigned long long* out_count);
+// `rounds`: the kernel walks cooperative rounds (cp_round_publish / cp_round_offset), so the single-wave mode also covers num_tiles >
+// resident_ctas.  Call it right before launch_compact(), which advances the ticket / arrival bookkeeping once the launch
+// is accepted.
+CompactScratch prepare_compact(const CtxPtr& ctx, long long num_tiles, long long resident_ctas, unsigned long long* out_count, bool rounds = false);
 
 // Launches a compaction kernel with sc.grid CTAs.  Single-wave launches wait for data of other CTAs, which only
 // arrives when EVERY CTA of the grid is running, so they go through the cooperative-launch path: the driver then
@@ -327,9 +389,19 @@ inline void launch_compact(const CtxPtr& ctx, Kernel kernel, const CompactScratc
 // Rank of survivor item k among the survivors of its tile (0 .. tile_total - 1) / its global output position.
 template <int E, int I>
 __device__ __forceinline__ unsigned cp_local_position(const CompactSmem<E, I>& s, unsigned long long bits, int k, const unsigned (&lane_prefix)[I / E]) {
+  constexpr int G = I / E;
   const int g = k / E, e = k % E;
   const unsigned within = __popcll(bits & (((1ull << e) - 1ull) << (g * E)));
-  return s.group_warp[g][threadIdx.x >> 5] + lane_prefix[g] + within;
+  unsigned lp;
+  if constexpr (G <= 8) {
+    // selects instead of a run-time index: the array stays in registers instead of going to local memory
+    lp = lane_prefix[0];
+#pragma unroll
+    for (int i = 1; i < G; ++i) lp = g == i ? lane_prefix[i] : lp;
+  } else {
+    lp = lane_prefix[g];
+  }
+  return s.group_warp[g][threadIdx.x >> 5] + lp + within;
 }
 
 template <int E, int I>

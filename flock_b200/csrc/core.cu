@@ -269,7 +269,7 @@ int scan_poll_sleep_ns() {
   return v;
 }
 
-CompactScratch prepare_compact(const CtxPtr& ctx, long long num_tiles, long long resident_ctas, unsigned long long* out_count) {
+CompactScratch prepare_compact(const CtxPtr& ctx, long long num_tiles, long long resident_ctas, unsigned long long* out_count, bool rounds) {
   ScanScratch& s = ctx->scan;
   const int stride = scan_stride();
   if (!s.ep_counters) {
@@ -307,7 +307,7 @@ CompactScratch prepare_compact(const CtxPtr& ctx, long long num_tiles, long long
   static const bool env_lookback = getenv("FLOCKGPU_FORCE_LOOKBACK") != nullptr;
   const bool force_lookback = env_lookback || ctx->compact_mode == 1;
   if (resident_ctas < 1) resident_ctas = 1;
-  sc.single_wave = (num_tiles <= resident_ctas && !force_lookback) ? 1 : 0;
+  sc.single_wave = ((rounds || num_tiles <= resident_ctas) && !force_lookback) ? 1 : 0;
   sc.grid = int(std::max<long long>(1, std::min<long long>(resident_ctas, num_tiles)));
   sc.stride = stride;
   sc.poll_sleep_ns = scan_poll_sleep_ns();

@@ -7,11 +7,11 @@
 //
 // filter_compact_kernel: ONE launch for the whole relation (all 64 Ki-row batches: a 1.3 MB batch is
 // 0.2 us of HBM traffic, far below launch latency, so per-batch launches cannot work).  CTAs take tiles of
-// 256 x {4, 16, 32, 64} rows (sized so that the relation is one wave of resident CTAs whenever possible),
-// evaluate the predicate (PredI32: one multiply-add + compare per row for the NEXMark shapes; the generic term
-// interpreter otherwise), rank the survivors (compact.cuh), obtain the tile's global output offset from the
-// grid-wide prefix protocol (each input byte is read once, no second pass), and write the surviving rows of every
-// fixed-width output column in input order.  Utf8 outputs leave through the selection vector and gather.cu.
+// 256 x {4, 16, 32} rows, evaluate the predicate (PredI32: one multiply-add + compare per row for the NEXMark shapes;
+// the generic term interpreter otherwise), rank the survivors (compact.cuh), obtain the tile's global output offset
+// from the grid-wide prefix protocol (each input byte is read once, no second pass), and write the surviving rows of
+// every fixed-width output column in input order.  PredI32 walks cooperative rounds with the next tile's column bytes
+// in flight (see the kernel).  Utf8 outputs leave through the selection vector and gather.cu.
 // Host-resident (page-locked, zero-copy fed) predicate columns are read in place over PCIe.
 #include <algorithm>
 #include <cstdlib>
@@ -41,7 +41,10 @@ struct FilterArgs {
 };
 
 // ---- predicate functors ---------------------------------------------------------------------------
-// A functor evaluates this thread's FP_ITEMS rows of a tile and returns one bit per item.  E = rows a
+// A functor evaluates this thread's I rows of a tile and returns one bit per item, in two steps: load() issues the
+// tile's loads into a Staged value (a shared-memory variable of the kernel) and test() turns it into the verdicts.
+// Between the two the kernel works on the previous tile, so a functor that stages asynchronous copies keeps them in
+// flight across that work.  E = rows a
 // thread loads contiguously (vector width); item k is row
 //   tile_base + ((k / E) * FP_THREADS + tid) * E + k % E.
 // ROWS = rows per thread per tile: 16 for large inputs; 4 for small ones, where 4 Ki-row tiles would leave most SMs
@@ -51,8 +54,11 @@ struct PredGenericT {
   static constexpr int E = 1;
   static constexpr int I = ROWS;
   static constexpr int MIN_CTAS = 1;
+  static constexpr bool ROUNDS = false;  // the interpreter's loads depend on each other: nothing to stage ahead
+  struct Staged {};
   Predicate p;
-  __device__ __forceinline__ unsigned long long eval(const ColRef* cols, int64_t tile_base, int64_t n_rows, int tid, int* err) const {
+  __device__ __forceinline__ void load(Staged&, int64_t, int64_t, int) const {}
+  __device__ __forceinline__ unsigned long long test(const Staged&, const ColRef* cols, int64_t tile_base, int64_t n_rows, int tid, int* err) const {
     int64_t rows[I];
 #pragma unroll
     for (int k = 0; k < I; ++k) {
@@ -64,11 +70,26 @@ struct PredGenericT {
 };
 
 
-template <int MODE, int ITEMS>
+// One tile = 8 Ki rows: every thread copies eight 16-byte pieces of the column per tile into shared memory with
+// cp.async, and the kernel keeps the next tile's copies in flight while it ranks, publishes and writes the current
+// one (cooperative rounds, compact.cuh).  Staging in shared memory instead of registers keeps the loads in flight
+// without costing registers, so more CTAs stay resident and each round covers more of the relation.
+__device__ __forceinline__ void cp_async16(void* smem, const void* gmem, int src_bytes) {
+  // src_bytes < 16 zero-fills the rest of the 16 bytes (rows past the end of the relation)
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(unsigned(__cvta_generic_to_shared(smem))), "l"(gmem), "r"(src_bytes)
+               : "memory");
+}
+
+template <int MODE>
 struct PredI32 {
   static constexpr int E = 4;
-  static constexpr int I = ITEMS;  // rows per thread per tile
-  static constexpr int MIN_CTAS = 5;  // <= 51 registers: 660 resident CTAs on 132 SMs, so 10 M rows (611 tiles) are one wave
+  static constexpr int L = 8;          // 16-byte copies per thread and tile
+  static constexpr int I = 4 * L;      // rows per thread per tile
+  static constexpr int MIN_CTAS = 4;   // <= 64 registers
+  static constexpr bool ROUNDS = true;
+  struct Staged {                      // in shared memory; thread t only touches v[.][t], so no barrier is needed
+    int4 v[L][FP_THREADS];
+  };
   const int32_t* col;
   PredI32Consts k;
   const void* const* chunks;  // host-resident column (zero-copy feed): chunk bases, else NULL
@@ -82,202 +103,260 @@ struct PredI32 {
   __device__ __forceinline__ unsigned test4(const int4& v) const {
     return unsigned(test(v.x)) | (unsigned(test(v.y)) << 1) | (unsigned(test(v.z)) << 2) | (unsigned(test(v.w)) << 3);
   }
-  // Streams the thread's rows in rounds of four 16-byte loads: only the one-bit verdicts are kept (the values of
-  // the ~1 % survivors are re-read from L2 when they are written), so the kernel needs ~48 registers and five CTAs
-  // stay resident per SM -- a 10 M-row relation (611 tiles of 16 Ki rows) is then a single wave.
-  __device__ __forceinline__ unsigned long long eval(const ColRef*, int64_t tile_base, int64_t n_rows, int tid, int*) const {
-    constexpr int L = 4;  // independent 16-byte loads in flight per thread and round (8 costs 80 registers = 3 CTAs/SM: no single wave)
-    constexpr int ROUNDS = I / (4 * L);
+  __device__ __forceinline__ void load(Staged& st, int64_t tile_base, int64_t n_rows, int tid) const {
     if (!chunks && tile_base + int64_t(FP_THREADS) * I <= n_rows) {
       // full tile of a device-resident column (every tile but the last): no bounds, no chunk lookup
       const int4* p = reinterpret_cast<const int4*>(col + tile_base) + tid;
-      unsigned half[2] = {0u, 0u};  // verdicts of rounds {0, 1} and {2, 3}: 32-bit shifts only
 #pragma unroll
-      for (int h = 0; h < (ROUNDS + 1) / 2; ++h) {
-#pragma unroll 1
-        for (int c = 2 * h; c < ROUNDS && c < 2 * h + 2; ++c) {
-          int4 v[L];
+      for (int j = 0; j < L; ++j) cp_async16(&st.v[j][tid], p + j * FP_THREADS, 16);
+    } else {
 #pragma unroll
-          for (int j = 0; j < L; ++j) v[j] = ldg_stream_v4(p + (c * L + j) * FP_THREADS);
-          unsigned b16 = 0;
-#pragma unroll
-          for (int j = 0; j < L; ++j) b16 |= test4(v[j]) << (4 * j);
-          half[h] |= b16 << (16 * (c & 1));
-        }
+      for (int j = 0; j < L; ++j) {
+        const int64_t row0 = tile_base + (int64_t(j) * FP_THREADS + tid) * 4;
+        const int64_t left = n_rows - row0;
+        cp_async16(&st.v[j][tid], at(left > 0 ? row0 : 0), left >= 4 ? 16 : left > 0 ? int(left) * 4 : 0);
       }
-      return (unsigned long long)half[0] | ((unsigned long long)half[1] << 32);
     }
-    unsigned long long bits = 0;
-#pragma unroll 1
-    for (int c = 0; c < ROUNDS; ++c) {
-      int4 v[L];
+    asm volatile("cp.async.commit_group;" ::: "memory");
+  }
+  // Only the one-bit verdicts outlive test(): the values of the ~1 % survivors are re-read from L2 when they are written.
+  __device__ __forceinline__ unsigned long long test(const Staged& st, const ColRef*, int64_t tile_base, int64_t n_rows, int tid, int*) const {
+    asm volatile("cp.async.wait_all;" ::: "memory");
+    unsigned bits = 0;
+#pragma unroll
+    for (int j = 0; j < L; ++j) bits |= test4(st.v[j][tid]) << (4 * j);
+    if (tile_base + int64_t(FP_THREADS) * I > n_rows) {
 #pragma unroll
       for (int j = 0; j < L; ++j) {
-        const int64_t row0 = tile_base + (int64_t(c * L + j) * FP_THREADS + tid) * 4;
-        if (row0 + 3 < n_rows) {
-          v[j] = ldg_stream_v4(at(row0));
-        } else {
-          v[j] = make_int4(0, 0, 0, 0);
-          if (row0 + 0 < n_rows) v[j].x = at(row0)[0];
-          if (row0 + 1 < n_rows) v[j].y = at(row0)[1];
-          if (row0 + 2 < n_rows) v[j].z = at(row0)[2];
-        }
-      }
-#pragma unroll
-      for (int j = 0; j < L; ++j) {
-        const int64_t row0 = tile_base + (int64_t(c * L + j) * FP_THREADS + tid) * 4;
-        unsigned b = test4(v[j]);
-        const int64_t left = n_rows - row0;  // mask rows past the end
-        if (left < 4) b &= left <= 0 ? 0u : ((1u << left) - 1u);
-        bits |= (unsigned long long)b << (4 * (c * L + j));
+        const int64_t left = n_rows - (tile_base + (int64_t(j) * FP_THREADS + tid) * 4);  // mask rows past the end
+        if (left < 4) bits &= ~((left <= 0 ? 0xfu : (0xfu << left) & 0xfu) << (4 * j));
       }
     }
     return bits;
   }
 };
 
-__device__ __forceinline__ void copy_value(void* dst, const void* src, int width, int64_t pos, int64_t row) {
-  if (width == 4) static_cast<uint32_t*>(dst)[pos] = static_cast<const uint32_t*>(src)[row];
-  else static_cast<uint64_t*>(dst)[pos] = static_cast<const uint64_t*>(src)[row];
+// Pulls the survivors' pass-through values (one dependent ~1 us DRAM read each) into L2 ahead of the write phase,
+// which then finds them there.  Every survivor is prefetched, not only the first four of a thread: in the cooperative
+// rounds a tile is written one whole iteration after it is ranked, so even a thread whose 32 rows all survive (the hot
+// auction id) has its values in L2 by then, and a prefetch costs the thread one instruction.
+template <int E>
+__device__ __forceinline__ void prefetch_survivors(const FilterArgs& a, unsigned long long bits, int64_t tile_base, int tid) {
+  if (!bits) return;
+  for (int c = 0; c < a.n_out; ++c) {
+    const OutCol& oc = a.outs[c];
+    if (oc.kind != OUT_PASS) continue;
+    const ColRef& src = a.cols[oc.src_col];
+    if (src.chunks) continue;  // host-resident: fetched once, when written
+    unsigned long long m = bits;
+#pragma unroll 1
+    while (m) {
+      const int k = __ffsll((long long)m) - 1;
+      m &= m - 1;
+      prefetch_l2(static_cast<const char*>(src.data) + (tile_base + cp_item_index<E>(k, tid)) * oc.width);
+    }
+  }
 }
 
-template <class PredFn>
-__global__ void __launch_bounds__(FP_THREADS, PredFn::MIN_CTAS) filter_compact_kernel(const __grid_constant__ PredFn pred, const __grid_constant__ FilterArgs a) {
+// Writes this thread's survivors of the tile to their output positions, in input order.  A thread may own many
+// survivors (NEXMark's hot auction id: when it satisfies the predicate half of the rows of a stretch survive), and
+// every pass-through value is a dependent ~1 us DRAM read: gather four survivors at a time so that their loads are in
+// flight together.  COMPUTED: some output is an expression (eval_chain), compiled only into the kernels that need it.
+template <int E, int I, bool COMPUTED>
+__device__ __forceinline__ void write_survivors(const FilterArgs& a, const CompactSmem<E, I>& sm, unsigned long long bits, int64_t tile_base,
+                                                const unsigned (&lane_prefix)[I / E], int tid, int* err) {
+  // positions and rows are kept as 32-bit offsets from the tile's output and input bases until used: the 64-bit
+  // forms of four survivors would not fit the register budget next to the next tile's loads in flight
+  const long long excl = (long long)sm.excl;
+  unsigned long long m = bits;
+  while (m) {
+    unsigned lpos[4], item[4];
+    int nb = 0;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      lpos[q] = 0;
+      item[q] = 0;
+      if (m) {
+        const int k = __ffsll((long long)m) - 1;
+        m &= m - 1;
+        lpos[q] = cp_local_position<E, I>(sm, bits, k, lane_prefix);
+        item[q] = unsigned(cp_item_index<E>(k, tid));
+        nb = q + 1;
+      }
+    }
+    if (a.sel_out) {
+#pragma unroll
+      for (int q = 0; q < 4; ++q)
+        if (q < nb) a.sel_out[excl + lpos[q]] = uint32_t(tile_base + item[q]);
+    }
+    for (int c = 0; c < a.n_out; ++c) {
+      const OutCol& oc = a.outs[c];
+      if (!COMPUTED || oc.kind == OUT_PASS) {
+        const ColRef& sc_col = a.cols[oc.src_col];
+        if (sc_col.chunks) {
+          // host-resident source: one PCIe read per survivor
+          const int64_t mask = (int64_t(1) << sc_col.chunk_shift) - 1;
+          uint64_t v[4];
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            v[q] = 0;
+            if (q < nb) {
+              const int64_t row = tile_base + item[q];
+              const char* base = static_cast<const char*>(sc_col.chunks[row >> sc_col.chunk_shift]) + (row & mask) * oc.width;
+              v[q] = oc.width == 4 ? uint64_t(*reinterpret_cast<const uint32_t*>(base)) : *reinterpret_cast<const uint64_t*>(base);
+            }
+          }
+#pragma unroll
+          for (int q = 0; q < 4; ++q)
+            if (q < nb) {
+              if (oc.width == 4) static_cast<uint32_t*>(oc.dst)[excl + lpos[q]] = uint32_t(v[q]);
+              else static_cast<uint64_t*>(oc.dst)[excl + lpos[q]] = v[q];
+            }
+        } else if (oc.width == 4) {
+          const uint32_t* src = static_cast<const uint32_t*>(sc_col.data) + tile_base;
+          uint32_t* dst = static_cast<uint32_t*>(oc.dst) + excl;
+          uint32_t v[4];
+#pragma unroll
+          for (int q = 0; q < 4; ++q) v[q] = q < nb ? src[item[q]] : 0u;
+#pragma unroll
+          for (int q = 0; q < 4; ++q)
+            if (q < nb) dst[lpos[q]] = v[q];
+        } else {
+          const uint64_t* src = static_cast<const uint64_t*>(sc_col.data) + tile_base;
+          uint64_t* dst = static_cast<uint64_t*>(oc.dst) + excl;
+          uint64_t v[4];
+#pragma unroll
+          for (int q = 0; q < 4; ++q) v[q] = q < nb ? src[item[q]] : 0ull;
+#pragma unroll
+          for (int q = 0; q < 4; ++q)
+            if (q < nb) dst[lpos[q]] = v[q];
+        }
+      } else if constexpr (COMPUTED) {
+        int64_t row[4];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) row[q] = q < nb ? tile_base + item[q] : -1;
+        Val acc[4];
+        eval_chain<4>(oc.chain, a.cols, row, acc, err);
+#pragma unroll
+        for (int q = 0; q < 4; ++q)
+          if (q < nb) store_val(oc.dst, oc.out_dtype, excl + lpos[q], acc[q]);
+      }
+    }
+  }
+}
+
+// Trace (FLOCKGPU_TRACE): 8 %globaltimer stamps per tile, written by thread 0 of the CTA that owns the tile:
+//   0 the CTA turns to the tile, 1 verdicts known (the tile's loads have landed), 2 ranked within the tile, 3 output
+//   offset known, 4 survivors written, 5 CTA end (its last tile only), 6 CTA index, 7 SM id.  In the cooperative
+//   rounds 3 and 4 come one iteration after 2: tile r is written after tile r + 1 is published.
+constexpr int FP_TRACE_WORDS = 8;
+
+// The expression interpreter of computed outputs needs more registers than MIN_CTAS allows: kernels that have it
+// trade residency for no spills (the cooperative rounds take any grid).
+template <class PredFn, bool COMPUTED>
+__global__ void __launch_bounds__(FP_THREADS, COMPUTED && PredFn::MIN_CTAS > 2 ? 2 : PredFn::MIN_CTAS) filter_compact_kernel(const __grid_constant__ PredFn pred, const __grid_constant__ FilterArgs a) {
   constexpr int E = PredFn::E;
   constexpr int I = PredFn::I;
   constexpr int TILE = FP_THREADS * I;
-  __shared__ CompactSmem<E, I> sm;
   const int tid = threadIdx.x;
   const CompactScratch& sc = a.sc;
   int err = 0;
 
-  auto stamp = [&](long long tile, int k) {
-    if (a.trace && tid == 0) {
-      unsigned long long t;
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-      a.trace[tile * 8 + k] = t;
-    }
+  auto now = [] {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
   };
-  unsigned long long t_begin = 0;
-  if (a.trace) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_begin));
-  long long tile;
-  for (int it = 0; (tile = cp_next_tile(sm, sc, it)) >= 0; ++it) {
-    const int64_t tile_base = tile * TILE;
-    if (a.trace && tid == 0) a.trace[tile * 8 + 0] = t_begin;
-    stamp(tile, 1);
-    const unsigned long long bits = pred.eval(a.cols, tile_base, a.n_rows, tid, &err);
-    stamp(tile, 2);
-    unsigned lane_prefix[I / E];
-    // While the CTA waits for the grid-wide prefix, pull the survivors' pass-through values (one dependent ~1 us
-    // DRAM read each) into L2: the write phase below then finds them there.
-    auto prefetch_survivors = [&] {
-      if (!bits) return;
-      for (int c = 0; c < a.n_out; ++c) {
-        const OutCol& oc = a.outs[c];
-        if (oc.kind != OUT_PASS) continue;
-        const ColRef& src = a.cols[oc.src_col];
-        if (src.chunks) continue;  // host-resident: fetched once, when written
-        unsigned long long m = bits;
-#pragma unroll 1
-        for (int q = 0; q < 4 && m; ++q) {
-          const int k = __ffsll((long long)m) - 1;
-          m &= m - 1;
-          prefetch_l2(static_cast<const char*>(src.data) + (tile_base + cp_item_index<E>(k, tid)) * oc.width);
-        }
-      }
-    };
-    cp_rank_tile<E, I>(sm, sc, tile, bits, lane_prefix, prefetch_survivors);
-    stamp(tile, 3);
-
-    // ---- write survivors in input order
-    // A thread may own many survivors (NEXMark's hot auction id: when it satisfies the predicate half of the rows
-    // of a stretch survive), and every pass-through value is a dependent ~1 us DRAM read: gather four survivors
-    // at a time so that their loads are in flight together.
-    if (bits && sm.tile_total) {
-      unsigned long long m = bits;
-      while (m) {
-        int64_t pos[4], row[4];
-        int nb = 0;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          pos[q] = 0;
-          row[q] = -1;
-          if (m) {
-            const int k = __ffsll((long long)m) - 1;
-            m &= m - 1;
-            pos[q] = cp_position<E, I>(sm, bits, k, lane_prefix);
-            row[q] = tile_base + cp_item_index<E>(k, tid);
-            nb = q + 1;
-          }
-        }
-        if (a.sel_out) {
-#pragma unroll
-          for (int q = 0; q < 4; ++q)
-            if (q < nb) a.sel_out[pos[q]] = uint32_t(row[q]);
-        }
-        for (int c = 0; c < a.n_out; ++c) {
-          const OutCol& oc = a.outs[c];
-          if (oc.kind == OUT_PASS) {
-            const ColRef& sc_col = a.cols[oc.src_col];
-            const void* src = sc_col.data;
-            if (sc_col.chunks) {
-              // host-resident source: one PCIe read per survivor
-              const int64_t mask = (int64_t(1) << sc_col.chunk_shift) - 1;
-              uint64_t v[4];
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                v[q] = 0;
-                if (q < nb) {
-                  const char* base = static_cast<const char*>(sc_col.chunks[row[q] >> sc_col.chunk_shift]) + (row[q] & mask) * oc.width;
-                  v[q] = oc.width == 4 ? uint64_t(*reinterpret_cast<const uint32_t*>(base)) : *reinterpret_cast<const uint64_t*>(base);
-                }
-              }
-#pragma unroll
-              for (int q = 0; q < 4; ++q)
-                if (q < nb) {
-                  if (oc.width == 4) static_cast<uint32_t*>(oc.dst)[pos[q]] = uint32_t(v[q]);
-                  else static_cast<uint64_t*>(oc.dst)[pos[q]] = v[q];
-                }
-            } else if (oc.width == 4) {
-              uint32_t v[4];
-#pragma unroll
-              for (int q = 0; q < 4; ++q) v[q] = q < nb ? static_cast<const uint32_t*>(src)[row[q]] : 0u;
-#pragma unroll
-              for (int q = 0; q < 4; ++q)
-                if (q < nb) static_cast<uint32_t*>(oc.dst)[pos[q]] = v[q];
-            } else {
-              uint64_t v[4];
-#pragma unroll
-              for (int q = 0; q < 4; ++q) v[q] = q < nb ? static_cast<const uint64_t*>(src)[row[q]] : 0ull;
-#pragma unroll
-              for (int q = 0; q < 4; ++q)
-                if (q < nb) static_cast<uint64_t*>(oc.dst)[pos[q]] = v[q];
-            }
-          } else {
-            Val acc[4];
-            eval_chain<4>(oc.chain, a.cols, row, acc, &err);
-#pragma unroll
-            for (int q = 0; q < 4; ++q)
-              if (q < nb) store_val(oc.dst, oc.out_dtype, pos[q], acc[q]);
-          }
-        }
-      }
-    }
-    __syncthreads();  // sm is reused by the next tile
-    stamp(tile, 4);
-    if (a.trace && tid == 0) a.trace[tile * 8 + 6] = blockIdx.x;
+  auto stamp = [&](long long tile, int k) {
+    if (a.trace && tid == 0) a.trace[tile * FP_TRACE_WORDS + k] = now();
+  };
+  auto stamp_ids = [&](long long tile) {
     if (a.trace && tid == 0) {
       unsigned smid;
       asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-      a.trace[tile * 8 + 7] = smid;
+      a.trace[tile * FP_TRACE_WORDS + 6] = blockIdx.x;
+      a.trace[tile * FP_TRACE_WORDS + 7] = smid;
     }
+  };
+
+  __shared__ typename PredFn::Staged st;
+  if (sc.single_wave) {
+    // Cooperative rounds (compact.cuh): tile blockIdx.x + r * grid in round r.  Iteration r tests tile r (its loads
+    // were issued one iteration earlier), issues tile r + 1's loads, ranks and publishes tile r, and only then reads
+    // the offset of tile r - 1 and writes its survivors.  So the loads stream while the CTA ranks, waits and writes,
+    // and a round's counts are published without waiting for anybody's writes.  Tile indices are 32-bit here (2^31
+    // tiles are far beyond any relation): 64-bit loop state would not fit the 64-register budget of four CTAs per SM.
+    __shared__ CompactSmem<E, I> rank_sm[2];  // tile r is ranked into rank_sm[r & 1] and written from it one iteration later
+    __shared__ unsigned long long rounds_done;
+    const int num_tiles = int(sc.num_tiles);
+    int tile = blockIdx.x;
+    if (tile < num_tiles) pred.load(st, int64_t(tile) * TILE, a.n_rows, tid);
+    // A thread's group prefixes are at most 31 x E < 256: the tile waiting for its writes keeps them as bytes (group g
+    // in byte g % 4 of register g / 4), which keeps the kernel within its register budget.
+    constexpr int G = I / E, P = (G + 3) / 4;
+    static_assert(31 * E < 256 && I <= 32, "group prefixes do not fit a byte, or verdicts a word");
+    unsigned prev_bits = 0, prev_packed[P] = {};
+    for (int it = 0;; ++it, tile += sc.grid) {
+      const int prev = tile - sc.grid;
+      unsigned bits = 0, packed[P] = {};
+      if (tile < num_tiles) {
+        stamp(tile, 0);
+        bits = unsigned(pred.test(st, a.cols, int64_t(tile) * TILE, a.n_rows, tid, &err));
+        stamp(tile, 1);
+        if (tile + sc.grid < num_tiles) pred.load(st, int64_t(tile + sc.grid) * TILE, a.n_rows, tid);
+        unsigned lane_prefix[I / E];
+        cp_rank_local<E, I>(rank_sm[it & 1], bits, lane_prefix);
+#pragma unroll
+        for (int g = 0; g < G; ++g) packed[g >> 2] |= lane_prefix[g] << ((g & 3) * 8);
+        stamp(tile, 2);
+        prefetch_survivors<E>(a, bits, int64_t(tile) * TILE, tid);
+        cp_round_publish(sc, tile, rank_sm[it & 1].tile_total);
+      }
+      if (it > 0) {
+        CompactSmem<E, I>& ps = rank_sm[(it - 1) & 1];
+        cp_round_offset<E, I>(ps, sc, prev, prev - int(blockIdx.x), rounds_done);
+        stamp(prev, 3);
+        if (prev_bits) {
+          unsigned prev_prefix[G];
+#pragma unroll
+          for (int g = 0; g < G; ++g) prev_prefix[g] = (prev_packed[g >> 2] >> ((g & 3) * 8)) & 0xffu;
+          write_survivors<E, I, COMPUTED>(a, ps, prev_bits, int64_t(prev) * TILE, prev_prefix, tid, &err);
+        }
+        __syncthreads();  // ps is reused by the next tile
+        stamp(prev, 4);
+        stamp_ids(prev);
+        if (tile >= num_tiles) stamp(prev, 5);
+      }
+      if (tile >= num_tiles) break;
+      prev_bits = bits;
+#pragma unroll
+      for (int i = 0; i < P; ++i) prev_packed[i] = packed[i];
+    }
+  } else {
+    // decoupled look-back: tiles drawn from the ticket counter, one at a time
+    __shared__ CompactSmem<E, I> sm;
+    long long tile, last = -1;
+    for (int it = 0; (tile = cp_next_tile(sm, sc, it)) >= 0; ++it) {
+      last = tile;
+      const int64_t tile_base = tile * TILE;
+      stamp(tile, 0);
+      pred.load(st, tile_base, a.n_rows, tid);
+      const unsigned long long bits = pred.test(st, a.cols, tile_base, a.n_rows, tid, &err);
+      stamp(tile, 1);
+      unsigned lane_prefix[I / E];
+      cp_rank_local<E, I>(sm, bits, lane_prefix);
+      stamp(tile, 2);
+      prefetch_survivors<E>(a, bits, tile_base, tid);
+      cp_block_lookback<E, I>(sm, sc, tile, sm.tile_total);
+      stamp(tile, 3);
+      if (bits) write_survivors<E, I, COMPUTED>(a, sm, bits, tile_base, lane_prefix, tid, &err);
+      __syncthreads();  // sm is reused by the next tile
+      stamp(tile, 4);
+      stamp_ids(tile);
+    }
+    if (last >= 0) stamp(last, 5);
   }
   if (err) *a.err_flag = 1;
-  if (a.trace && tid == 0) {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    a.trace[(long long)blockIdx.x * 8 + 5] = t;   // per CTA (indexed by block, not tile)
-  }
 }
 
 // ---- pure projection (no predicate): streaming evaluation of the computed columns ----------------
@@ -365,36 +444,41 @@ static void fill_colrefs(const Table& t, ColRef* refs) {
   }
 }
 
-template <class PredFn>
+// Launches the filter over the whole relation in tiles of FP_THREADS x PredFn::I rows.  The grid is the resident CTAs
+// of the instantiation launched: functors with ROUNDS walk any number of cooperative rounds; the others run one
+// wave when the tiles fit it and fall back to decoupled look-back beyond it.
+template <class PredFn, bool COMPUTED>
 static void launch_filter(const CtxPtr& ctx, const PredFn& pred, FilterArgs args) {
   constexpr int64_t TILE = int64_t(FP_THREADS) * PredFn::I;
   const int64_t num_tiles = (args.n_rows + TILE - 1) / TILE;
-  const void* k = reinterpret_cast<const void*>(&filter_compact_kernel<PredFn>);
-  args.sc = prepare_compact(ctx, num_tiles, resident_ctas(ctx, k, FP_THREADS), args.out_count);
+  auto* kernel = &filter_compact_kernel<PredFn, COMPUTED>;
+  args.sc = prepare_compact(ctx, num_tiles, resident_ctas(ctx, reinterpret_cast<const void*>(kernel), FP_THREADS), args.out_count, PredFn::ROUNDS);
   const int grid = args.sc.grid;
   args.sc.host_count = args.host_count;
   BufferPtr trace_buf;
   static const char* trace_path = getenv("FLOCKGPU_TRACE");
+  const size_t trace_words = size_t(num_tiles) * FP_TRACE_WORDS;
   if (trace_path) {
-    trace_buf = alloc(ctx, size_t(num_tiles + 2048) * 64);
-    FG_CUDA(cudaMemsetAsync(trace_buf->ptr, 0, size_t(num_tiles + 2048) * 64, ctx->stream));
+    trace_buf = alloc(ctx, trace_words * 8);
+    FG_CUDA(cudaMemsetAsync(trace_buf->ptr, 0, trace_words * 8, ctx->stream));
     args.trace = trace_buf->as<unsigned long long>();
   }
   {
     LaunchTimer lt(ctx, "filter_compact_kernel");
-    launch_compact(ctx, filter_compact_kernel<PredFn>, args.sc, pred, args);
+    launch_compact(ctx, kernel, args.sc, pred, args);
   }
   FG_CUDA(cudaGetLastError());
   count_launch(ctx);
   if (trace_path) {
-    // debug only: dump the per-tile time stamps of this launch (overwrites the file each launch)
-    std::vector<unsigned long long> h(size_t(num_tiles + 2048) * 8);
+    // debug only: dump the per-tile time stamps of this launch (overwrites the file each launch).  Header: tiles, grid,
+    // 1 when tile t ran in round t / grid of the cooperative mode (0: decoupled look-back).
+    std::vector<unsigned long long> h(trace_words);
     FG_CUDA(cudaMemcpyAsync(h.data(), trace_buf->ptr, h.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
     FG_CUDA(cudaStreamSynchronize(ctx->stream));
     if (FILE* f = fopen(trace_path, "w")) {
-      fprintf(f, "%lld %d\n", (long long)num_tiles, grid);
-      for (size_t i = 0; i < h.size() / 8; ++i) {
-        for (int j = 0; j < 8; ++j) fprintf(f, "%llu ", h[i * 8 + j]);
+      fprintf(f, "%lld %d %d\n", (long long)num_tiles, grid, args.sc.single_wave);
+      for (size_t i = 0; i < h.size() / FP_TRACE_WORDS; ++i) {
+        for (int j = 0; j < FP_TRACE_WORDS; ++j) fprintf(f, "%llu ", h[i * FP_TRACE_WORDS + j]);
         fprintf(f, "\n");
       }
       fclose(f);
@@ -651,18 +735,14 @@ TablePtr filter_project(const CtxPtr& ctx, const TablePtr& in_ptr, const Expr* p
     if (pending) pending->h2d_bytes_per_row = zc_bytes_per_survivor;
   }
 
-  // rows per thread per tile of the vectorised functors (FLOCKGPU_FILTER_ITEMS = 16 | 32 | 64 overrides, for tuning)
-  // The smallest tile that still keeps the relation a single wave (<= ~700 tiles of 256 x items rows): small inputs
-  // spread over more SMs, 10 M-row relations use 64.
-  static const int items_env = [] {
-    const char* e = getenv("FLOCKGPU_FILTER_ITEMS");
-    int v = e ? atoi(e) : 0;
-    return (v == 16 || v == 32 || v == 64) ? v : 0;
-  }();
-  const int64_t single_wave_tiles = std::max<int64_t>(64, int64_t(ctx->sm_count) * 5 - 40);
-  const int items = items_env ? items_env
-                    : in.num_rows <= single_wave_tiles * FP_THREADS * 16 ? 16
-                    : in.num_rows <= single_wave_tiles * FP_THREADS * 32 ? 32 : 64;
+  // computed outputs (eval_chain) are compiled only into the kernels that have them
+  bool computed = false;
+  for (int c = 0; c < fa.n_out; ++c) computed |= fa.outs[c].kind != OUT_PASS;
+  auto launch = [&](const auto& pred) {
+    using PredFn = std::decay_t<decltype(pred)>;
+    if (computed) launch_filter<PredFn, true>(ctx, pred, fa);
+    else launch_filter<PredFn, false>(ctx, pred, fa);
+  };
   auto launch_i32 = [&](int64_t modulus) {
     const Column& pc = in.cols[cp.fast.col];
     const int32_t* col = static_cast<const int32_t*>(pc.values());
@@ -670,15 +750,9 @@ TablePtr filter_project(const CtxPtr& ctx, const TablePtr& in_ptr, const Expr* p
     const int32_t chunk_shift = pc.chunks ? pc.chunks->shift : 0;
     PredI32Consts k;
     const int mode = pred_i32_consts(modulus, cp.fast.cmp, cp.fast.rhs, &k);
-    auto go = [&](auto mode_tag) {
-      constexpr int MODE = decltype(mode_tag)::value;
-      if (items == 16) launch_filter(ctx, PredI32<MODE, 16>{col, k, chunks, chunk_shift}, fa);
-      else if (items == 32) launch_filter(ctx, PredI32<MODE, 32>{col, k, chunks, chunk_shift}, fa);
-      else launch_filter(ctx, PredI32<MODE, 64>{col, k, chunks, chunk_shift}, fa);
-    };
-    if (mode == 0) go(std::integral_constant<int, 0>{});
-    else if (mode == 1) go(std::integral_constant<int, 1>{});
-    else go(std::integral_constant<int, 2>{});
+    if (mode == 0) launch(PredI32<0>{col, k, chunks, chunk_shift});
+    else if (mode == 1) launch(PredI32<1>{col, k, chunks, chunk_shift});
+    else launch(PredI32<2>{col, k, chunks, chunk_shift});
   };
   switch (cp.fast.kind) {
     case FAST_PRED_I32_MOD_CMP:
@@ -688,8 +762,8 @@ TablePtr filter_project(const CtxPtr& ctx, const TablePtr& in_ptr, const Expr* p
       launch_i32(0);
       break;
     default: {
-      if (in.num_rows >= int64_t(ctx->sm_count) * 4 * FP_THREADS * 16) launch_filter(ctx, PredGenericT<16>{cp.prog}, fa);
-      else launch_filter(ctx, PredGenericT<4>{cp.prog}, fa);
+      if (in.num_rows >= int64_t(ctx->sm_count) * 4 * FP_THREADS * 16) launch(PredGenericT<16>{cp.prog});
+      else launch(PredGenericT<4>{cp.prog});
     }
   }
 

@@ -1,5 +1,9 @@
 #!/usr/bin/env python
-"""Debug: per-tile globaltimer stamps of filter_compact_kernel on the q2 workload (FLOCKGPU_TRACE=<file>)."""
+"""Debug: per-tile globaltimer stamps of filter_compact_kernel on the q2 workload (FLOCKGPU_TRACE=<file>), per round.
+
+Round r of the cooperative mode is the band of tiles [r * grid, (r + 1) * grid).  Times are microseconds from the first
+CTA start.  "wait loads" is how long a tile's verdicts came after the CTA finished its previous tile: about zero when
+the tile's loads, issued one round earlier, landed while that round ranked, waited for its prefix and wrote."""
 import os, sys
 from pathlib import Path
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
@@ -15,22 +19,26 @@ for i in range(6):
     ec.feed_tables([tabs[i % 3]])
     n = ec.execute_device(0).num_rows
 rows = [l.split() for l in open(out).read().splitlines()]
-ntiles, grid = int(rows[0][0]), int(rows[0][1])
+ntiles, grid, rounds_mode = int(rows[0][0]), int(rows[0][1]), int(rows[0][2])
 a = np.array([[int(x) for x in r] for r in rows[1:1 + ntiles]], dtype=np.int64)
-blk_end = np.array([int(r[5]) for r in rows[1:1 + grid]], dtype=np.int64)
 t0 = a[:, 0].min()
-def stat(x): return f"min {x.min()/1e3:7.2f}  p50 {np.median(x)/1e3:7.2f}  p90 {np.percentile(x,90)/1e3:7.2f}  max {x.max()/1e3:7.2f} us"
-print("tiles", ntiles, "grid", grid, "rows kept", n)
-print("cta start   ", stat(a[:, 0] - t0))
-print("got ticket  ", stat(a[:, 1] - t0))
-print("loaded+eval ", stat(a[:, 2] - t0))
-print("ranked+lb   ", stat(a[:, 3] - t0))
-print("written     ", stat(a[:, 4] - t0))
-print("cta end     ", stat(blk_end[blk_end > 0] - t0))
-print("load phase  ", stat(a[:, 2] - a[:, 1]))
-print("rank+lookbk ", stat(a[:, 3] - a[:, 2]))
-print("write phase ", stat(a[:, 4] - a[:, 3]))
+us = lambda x: (x - t0) / 1e3
+def stat(x): return f"min {x.min():7.2f}  p50 {np.median(x):7.2f}  max {x.max():7.2f}"
+print("tiles", ntiles, "grid", grid, "cooperative rounds" if rounds_mode else "decoupled look-back", "rows kept", n)
+rnd = np.arange(ntiles) // grid if rounds_mode else np.zeros(ntiles, dtype=np.int64)
+for r in range(rnd.max() + 1):
+    s = a[rnd == r]
+    print(f"round {r} ({len(s)} tiles)")
+    print("  start        ", stat(us(s[:, 0])))
+    print("  verdicts     ", stat(us(s[:, 1])))
+    print("  ranked       ", stat(us(s[:, 2])))
+    print("  prefix known ", stat(us(s[:, 3])))
+    print("  written      ", stat(us(s[:, 4])))
+    print("  wait loads   ", stat((s[:, 1] - s[:, 0]) / 1e3))
+    print("  rank->offset ", stat((s[:, 3] - s[:, 2]) / 1e3))
+    print("  write phase  ", stat((s[:, 4] - s[:, 3]) / 1e3))
+end = a[a[:, 5] > 0, 5]
+if len(end):
+    print("cta end        ", stat(us(end)))
 sm = a[:, 7]
 print("tiles per SM: min", np.bincount(sm).min(), "max", np.bincount(sm).max())
-order = np.argsort(a[:, 2])
-print("tile index of the 10 last-loaded tiles:", order[-10:], "their load-done times", (a[order[-10:], 2] - t0) / 1e3)
