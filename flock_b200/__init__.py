@@ -38,6 +38,9 @@ AGG_PARTIAL, AGG_FINAL, AGG_FINAL_PARTITIONED, AGG_SINGLE = 0, 1, 2, 3
 AGG_COUNT, AGG_SUM, AGG_MIN, AGG_MAX, AGG_AVG = 0, 1, 2, 3, 4
 _AGG_BY_NAME = {"count": AGG_COUNT, "sum": AGG_SUM, "min": AGG_MIN, "max": AGG_MAX, "avg": AGG_AVG}
 _MODE_BY_NAME = {"partial": AGG_PARTIAL, "final": AGG_FINAL, "final_partitioned": AGG_FINAL_PARTITIONED, "single": AGG_SINGLE}
+# FLOCKGPU_ENCODING_*: the discriminants of Flock's `Encoding` (flock/src/encoding.rs)
+ENCODING_SNAPPY, ENCODING_LZ4, ENCODING_ZLIB, ENCODING_ZSTD, ENCODING_NONE = 0, 1, 2, 3, 4
+ENCODINGS = {"snappy": ENCODING_SNAPPY, "lz4": ENCODING_LZ4, "zlib": ENCODING_ZLIB, "zstd": ENCODING_ZSTD, "none": ENCODING_NONE}
 
 
 # ------------------------------------------------------------------------------------------------
@@ -342,6 +345,32 @@ class Context:
                 C.CFUNCTYPE(None, C.c_void_p)(c_schema.release)(C.addressof(c_schema))
         return Table(self, out.value)
 
+    def import_payload(self, schema: pa.Schema, frames: Sequence[tuple], projection: Sequence[int] | None = None,
+                       encoding: str = "zstd") -> Table:
+        """frames: [(header, body)] of a payload as Flock sends it, each part compressed with `encoding` (Flock's `Encoding`:
+        "zstd", its default, or "none"; "snappy" / "lz4" / "zlib" raise FlockGpuError(ERR_UNSUPPORTED)).  zstd bodies are
+        decoded on the GPU (flockgpu_table_import_payload)."""
+        code = ENCODINGS.get(encoding, encoding) if isinstance(encoding, str) else int(encoding)
+        if not isinstance(code, int):
+            raise ValueError(f"unknown encoding {encoding!r}; one of {sorted(ENCODINGS)}")
+        n = len(frames)
+        keep = [(pa.py_buffer(h) if not isinstance(h, pa.Buffer) else h, pa.py_buffer(b) if not isinstance(b, pa.Buffer) else b) for h, b in frames]
+        hp = (C.c_void_p * max(n, 1))(*[h.address for h, _ in keep])
+        hl = (C.c_int64 * max(n, 1))(*[h.size for h, _ in keep])
+        bp = (C.c_void_p * max(n, 1))(*[b.address for _, b in keep])
+        bl = (C.c_int64 * max(n, 1))(*[b.size for _, b in keep])
+        c_schema = _ffi.ArrowSchema()
+        schema._export_to_c(C.addressof(c_schema))
+        try:
+            proj = (C.c_int32 * len(projection))(*projection) if projection is not None else None
+            out = C.c_void_p()
+            check(lib.flockgpu_table_import_payload(self.handle, C.byref(c_schema), code, hp, hl, bp, bl, n, proj,
+                                                    len(projection) if projection is not None else 0, C.byref(out)))
+        finally:
+            if c_schema.release:
+                C.CFUNCTYPE(None, C.c_void_p)(c_schema.release)(C.addressof(c_schema))
+        return Table(self, out.value)
+
     def import_ndjson(self, schema: pa.Schema, text: bytes) -> Table:
         """One flat JSON object per line -> table (event_bytes_to_batch, flock/src/transmute.rs:255-266)."""
         buf = pa.py_buffer(text)
@@ -497,6 +526,16 @@ def selftest_eval_predicate(batch: pa.RecordBatch, predicate: E):
     finally:
         _release_exported(c_schema, arrays, 1)
     return mask[:batch.num_rows].astype(bool), fast.value
+
+
+def selftest_zstd_decompress(data: bytes, capacity: int) -> bytes:
+    """CPU-only: decodes a zstd stream with the decoder functions of the GPU payload import (csrc/zstd_dec.h), serially on
+    the host.  Raises FlockGpuError(ERR_INVALID) on malformed input or more than `capacity` decoded bytes."""
+    src = pa.py_buffer(data)
+    dst = C.create_string_buffer(max(capacity, 1))
+    n = C.c_int64()
+    check(lib.flockgpu_selftest_zstd_decompress(C.c_void_p(src.address), src.size, dst, capacity, C.byref(n)))
+    return dst.raw[:n.value]
 
 
 def selftest_pred_i32(x, modulus: int, cmp: int, rhs: int):

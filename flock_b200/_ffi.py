@@ -126,6 +126,8 @@ PROTOTYPES = {
     "flockgpu_table_schema": (C.c_int, [_P, _P, C.POINTER(ArrowSchema)]),
     "flockgpu_table_import_ipc": (C.c_int, [_P, C.POINTER(ArrowSchema), C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(C.c_void_p),
                                            C.POINTER(C.c_int64), C.c_int32, _I32P, C.c_int32, _PP]),
+    "flockgpu_table_import_payload": (C.c_int, [_P, C.POINTER(ArrowSchema), C.c_int32, C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(C.c_void_p),
+                                               C.POINTER(C.c_int64), C.c_int32, _I32P, C.c_int32, _PP]),
     "flockgpu_table_export_ipc": (C.c_int, [_P, _P, C.c_int64, C.c_int64, _PP, C.POINTER(C.c_int64), _PP, C.POINTER(C.c_int64)]),
     "flockgpu_ipc_free": (None, [_P]),
     "flockgpu_table_import_ndjson": (C.c_int, [_P, C.POINTER(ArrowSchema), _P, C.c_int64, _PP]),
@@ -164,6 +166,7 @@ PROTOTYPES = {
     "flock_context_plan_str": (C.c_char_p, [_P, C.c_int32]),
     "flockgpu_selftest_eval_predicate": (C.c_int, [C.POINTER(ArrowSchema), C.POINTER(ArrowArray), C.POINTER(Expr), _P, _I32P]),
     "flockgpu_selftest_eval_value": (C.c_int, [C.POINTER(ArrowSchema), C.POINTER(ArrowArray), C.POINTER(Expr), _P, _I32P, _I32P]),
+    "flockgpu_selftest_zstd_decompress": (C.c_int, [_P, C.c_int64, _P, C.c_int64, C.POINTER(C.c_int64)]),
     "flockgpu_selftest_pred_i32": (C.c_int, [C.c_int64, C.c_int32, C.c_int64, _I32P, C.c_int64, C.POINTER(C.c_uint8), _I32P]),
 }
 

@@ -462,7 +462,7 @@ static bool range_has_null(const uint8_t* bitmap, int64_t off, int64_t len) {
   return false;
 }
 
-static std::string copy_metadata(const char* md) {
+std::string copy_metadata(const char* md) {
   // Arrow metadata block: int32 n, then n x (int32 klen, key, int32 vlen, value)
   if (!md) return std::string();
   const char* p = md;
@@ -611,6 +611,83 @@ void* pin_get(size_t bytes);
 void pin_put(void* p, size_t bytes);
 }  // namespace
 
+namespace {
+// Page-locked staging blocks of one import; they return to the cache when the import is done with them.
+struct PinnedBlocks {
+  std::vector<std::pair<void*, size_t>> v;
+  void emplace_back(void* p, size_t n) { v.emplace_back(p, n); }
+  ~PinnedBlocks() {
+    for (auto& b : v) pin_put(b.first, b.second);
+  }
+};
+
+// Issues the host -> device copies of `pieces` (fixed_bytes in all) on the copy streams and joins them into the main
+// stream.  The staging blocks it takes go to `staged`: the caller keeps them until the copies have drained.
+void issue_pieces(const CtxPtr& ctx, CopyFan& fan, const std::vector<HostPiece>& pieces, size_t fixed_bytes, PinnedBlocks& staged) {
+  fan.fork();
+  const int n_thr = int(std::min<size_t>(size_t(ctx->feed_stage_threads), pieces.size()));
+  if (n_thr >= 1 && fixed_bytes >= (size_t(1) << 20) && is_pageable(pieces[0].src)) {
+    // Pageable sources (what arrow-rs hands over): cudaMemcpyAsync would bounce every batch through the driver's own
+    // staging buffer on ONE thread.  Host threads copy the batches into a page-locked block instead and each issues
+    // the DMA of a batch as soon as it has copied it, so the host copies run in parallel with each other and with
+    // the link.
+    char* stage = static_cast<char*>(pin_get(fixed_bytes));
+    staged.emplace_back(stage, fixed_bytes);
+    // DMA chunks: runs of consecutive pieces that are contiguous on both sides (one column's batches), about 4 MB
+    // each.  The workers only copy; THIS thread issues a chunk's DMA as soon as its last piece has been staged
+    // (one cudaMemcpyAsync per chunk: 306 per-batch calls from many threads serialised on the driver's lock).
+    struct Chunk {
+      char* dst;
+      size_t stage_off, bytes;
+      int pieces;
+    };
+    std::vector<Chunk> chunks;
+    std::vector<int> chunk_of(pieces.size());
+    for (size_t i = 0; i < pieces.size(); ++i) {
+      const bool extend = !chunks.empty() && chunks.back().dst + chunks.back().bytes == pieces[i].dst &&
+                          chunks.back().stage_off + chunks.back().bytes == pieces[i].stage_off && chunks.back().bytes < (size_t(4) << 20);
+      if (!extend) chunks.push_back({pieces[i].dst, pieces[i].stage_off, 0, 0});
+      chunks.back().bytes += pieces[i].bytes;
+      chunks.back().pieces += 1;
+      chunk_of[i] = int(chunks.size()) - 1;
+    }
+    std::unique_ptr<std::atomic<int>[]> remaining(new std::atomic<int>[chunks.size()]);
+    for (size_t c = 0; c < chunks.size(); ++c) remaining[c].store(chunks[c].pieces);
+    std::atomic<size_t> next{0};
+    const int stream_stores = ctx->feed_stream_stores;
+    const std::function<void()> worker = [&]() {
+      for (size_t i = next.fetch_add(1); i < pieces.size(); i = next.fetch_add(1)) {
+        stage_copy(stage + pieces[i].stage_off, pieces[i].src, pieces[i].bytes, stream_stores);
+        remaining[chunk_of[i]].fetch_sub(1, std::memory_order_release);
+      }
+    };
+    ctx->stage_pool.start(n_thr, &worker);
+    cudaError_t issue_err = cudaSuccess;
+    for (size_t c = 0; c < chunks.size(); ++c) {
+      while (remaining[c].load(std::memory_order_acquire) > 0) {
+      }
+      cudaError_t e = cudaMemcpyAsync(chunks[c].dst, stage + chunks[c].stage_off, chunks[c].bytes, cudaMemcpyHostToDevice,
+                                      ctx->copy_streams[c % CtxCore::kCopyStreams]);
+      if (e != cudaSuccess && issue_err == cudaSuccess) issue_err = e;
+    }
+    ctx->stage_pool.wait();
+    FG_CHECK(issue_err == cudaSuccess, FLOCKGPU_ERR_CUDA, "table_import: staged host-to-device copy failed: %s", cudaGetErrorString(issue_err));
+    for (int i = 0; i < CtxCore::kCopyStreams; ++i) fan.used[i] = true;
+    ctx->h2d_bytes.fetch_add(int64_t(fixed_bytes), std::memory_order_relaxed);
+  } else {
+    for (const HostPiece& pc : pieces) fan.copy(pc.dst, pc.src, pc.bytes);
+  }
+  fan.join();
+}
+}  // namespace
+
+void upload_host_pieces(const CtxPtr& ctx, const std::vector<HostPiece>& pieces, size_t total_bytes) {
+  CopyFan fan(ctx);
+  PinnedBlocks staged;
+  if (!pieces.empty()) issue_pieces(ctx, fan, pieces, total_bytes, staged);
+  FG_CUDA(cudaStreamSynchronize(ctx->stream));
+}
+
 TablePtr import_batches(const CtxPtr& ctx, const ArrowSchema* schema, const ArrowArray* const* batches,
                         int n_batches, const int* projection, int n_projection, bool zero_copy) {
   FG_CHECK(schema && schema->format && !strcmp(schema->format, "+s"), FLOCKGPU_ERR_INVALID,
@@ -624,13 +701,7 @@ TablePtr import_batches(const CtxPtr& ctx, const ArrowSchema* schema, const Arro
   }
   CopyFan fan(ctx);
   // page-locked staging blocks of this call (pageable sources); they return to the cache once the copies have drained
-  struct StagedBlocks {
-    std::vector<std::pair<void*, size_t>> v;
-    void emplace_back(void* p, size_t n) { v.emplace_back(p, n); }
-    ~StagedBlocks() {
-      for (auto& b : v) pin_put(b.first, b.second);
-    }
-  } staged;
+  PinnedBlocks staged;
   int64_t total = 0;
   for (int b = 0; b < n_batches; ++b) {
     FG_CHECK(batches[b] && batches[b]->n_children == schema->n_children, FLOCKGPU_ERR_INVALID,
@@ -646,13 +717,7 @@ TablePtr import_batches(const CtxPtr& ctx, const ArrowSchema* schema, const Arro
   t->num_rows = total;
   t->metadata = copy_metadata(schema->metadata);
   // host -> device copies of the fixed-width columns: collected for ALL columns, then issued together
-  struct Piece {
-    char* dst;
-    const char* src;
-    size_t bytes;
-    size_t stage_off;
-  };
-  std::vector<Piece> pieces;
+  std::vector<HostPiece> pieces;
   size_t fixed_bytes = 0;
   std::shared_ptr<HostRegistration> registration;
   if (zero_copy && ctx->feed_register && total > 0) {
@@ -755,62 +820,7 @@ TablePtr import_batches(const CtxPtr& ctx, const ArrowSchema* schema, const Arro
     }
     t->cols.push_back(std::move(col));
   }
-  if (!pieces.empty()) {
-    fan.fork();
-    const int n_thr = int(std::min<size_t>(size_t(ctx->feed_stage_threads), pieces.size()));
-    if (n_thr >= 1 && fixed_bytes >= (size_t(1) << 20) && is_pageable(pieces[0].src)) {
-      // Pageable sources (what arrow-rs hands over): cudaMemcpyAsync would bounce every batch through the driver's own
-      // staging buffer on ONE thread.  Host threads copy the batches into a page-locked block instead and each issues
-      // the DMA of a batch as soon as it has copied it, so the host copies run in parallel with each other and with
-      // the link.
-      char* stage = static_cast<char*>(pin_get(fixed_bytes));
-      staged.emplace_back(stage, fixed_bytes);
-      // DMA chunks: runs of consecutive pieces that are contiguous on both sides (one column's batches), about 4 MB
-      // each.  The workers only copy; THIS thread issues a chunk's DMA as soon as its last piece has been staged
-      // (one cudaMemcpyAsync per chunk: 306 per-batch calls from many threads serialised on the driver's lock).
-      struct Chunk {
-        char* dst;
-        size_t stage_off, bytes;
-        int pieces;
-      };
-      std::vector<Chunk> chunks;
-      std::vector<int> chunk_of(pieces.size());
-      for (size_t i = 0; i < pieces.size(); ++i) {
-        const bool extend = !chunks.empty() && chunks.back().dst + chunks.back().bytes == pieces[i].dst &&
-                            chunks.back().stage_off + chunks.back().bytes == pieces[i].stage_off && chunks.back().bytes < (size_t(4) << 20);
-        if (!extend) chunks.push_back({pieces[i].dst, pieces[i].stage_off, 0, 0});
-        chunks.back().bytes += pieces[i].bytes;
-        chunks.back().pieces += 1;
-        chunk_of[i] = int(chunks.size()) - 1;
-      }
-      std::unique_ptr<std::atomic<int>[]> remaining(new std::atomic<int>[chunks.size()]);
-      for (size_t c = 0; c < chunks.size(); ++c) remaining[c].store(chunks[c].pieces);
-      std::atomic<size_t> next{0};
-      const int stream_stores = ctx->feed_stream_stores;
-      const std::function<void()> worker = [&]() {
-        for (size_t i = next.fetch_add(1); i < pieces.size(); i = next.fetch_add(1)) {
-          stage_copy(stage + pieces[i].stage_off, pieces[i].src, pieces[i].bytes, stream_stores);
-          remaining[chunk_of[i]].fetch_sub(1, std::memory_order_release);
-        }
-      };
-      ctx->stage_pool.start(n_thr, &worker);
-      cudaError_t issue_err = cudaSuccess;
-      for (size_t c = 0; c < chunks.size(); ++c) {
-        while (remaining[c].load(std::memory_order_acquire) > 0) {
-        }
-        cudaError_t e = cudaMemcpyAsync(chunks[c].dst, stage + chunks[c].stage_off, chunks[c].bytes, cudaMemcpyHostToDevice,
-                                        ctx->copy_streams[c % CtxCore::kCopyStreams]);
-        if (e != cudaSuccess && issue_err == cudaSuccess) issue_err = e;
-      }
-      ctx->stage_pool.wait();
-      FG_CHECK(issue_err == cudaSuccess, FLOCKGPU_ERR_CUDA, "table_import: staged host-to-device copy failed: %s", cudaGetErrorString(issue_err));
-      for (int i = 0; i < CtxCore::kCopyStreams; ++i) fan.used[i] = true;
-      ctx->h2d_bytes.fetch_add(int64_t(fixed_bytes), std::memory_order_relaxed);
-    } else {
-      for (const Piece& pc : pieces) fan.copy(pc.dst, pc.src, pc.bytes);
-    }
-    fan.join();
-  }
+  if (!pieces.empty()) issue_pieces(ctx, fan, pieces, fixed_bytes, staged);
   // inputs are only borrowed for the call: every copy must have left the host buffers before we return
   FG_CUDA(cudaStreamSynchronize(ctx->stream));
   return t;

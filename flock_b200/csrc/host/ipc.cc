@@ -47,11 +47,7 @@ struct Fb {
   size_t indirect(size_t at) const { return at + rd<uint32_t>(at); }
 };
 
-struct FrameLayout {
-  int64_t length = 0;
-  std::vector<std::pair<int64_t, int64_t>> nodes;    // (length, null_count) per field
-  std::vector<std::pair<int64_t, int64_t>> buffers;  // (offset, length) into the body
-};
+}  // namespace
 
 FrameLayout parse_record_batch_message(const uint8_t* header, int64_t header_len) {
   FG_CHECK(header && header_len >= 8, FLOCKGPU_ERR_INVALID, "IPC header: empty");
@@ -59,10 +55,11 @@ FrameLayout parse_record_batch_message(const uint8_t* header, int64_t header_len
   const size_t msg = fb.indirect(0);
   const size_t f_type = fb.field(msg, 1), f_header = fb.field(msg, 2);
   FG_CHECK(f_type && f_header, FLOCKGPU_ERR_INVALID, "IPC header: Message without a header union");
+  FrameLayout L;
   const uint8_t type = fb.rd<uint8_t>(f_type);
   FG_CHECK(type == 3, FLOCKGPU_ERR_UNSUPPORTED, "IPC header: message type %d (only RecordBatch = 3 frames carry data; dictionaries are not supported)", int(type));
+  if (size_t f = fb.field(msg, 3)) L.body_length = fb.rd<int64_t>(f);
   const size_t rb = fb.indirect(f_header);
-  FrameLayout L;
   if (size_t f = fb.field(rb, 0)) L.length = fb.rd<int64_t>(f);
   FG_CHECK(!fb.field(rb, 3), FLOCKGPU_ERR_UNSUPPORTED, "IPC header: compressed record batch bodies (BodyCompression) are not supported");
   if (size_t f = fb.field(rb, 1)) {
@@ -77,6 +74,8 @@ FrameLayout parse_record_batch_message(const uint8_t* header, int64_t header_len
   }
   return L;
 }
+
+namespace {
 
 // ---- writing the header of one record batch --------------------------------------------------------------------------------
 struct Out {
@@ -135,6 +134,55 @@ std::vector<uint8_t> build_record_batch_message(int64_t length, const std::vecto
 
 }  // namespace
 
+// Everything about frame `f` that its header alone decides, against the schema and a body of `body_len` bytes: field
+// count, batch and field lengths, null counts, and every buffer extent.  The Utf8 offsets live in the body; the caller
+// checks them (check_utf8_extent).
+void check_frame_layout(const ArrowSchema* schema, int f, const FrameLayout& L, int64_t body_len) {
+  const int64_t n_fields = schema->n_children;
+  FG_CHECK(int64_t(L.nodes.size()) == n_fields, FLOCKGPU_ERR_INVALID, "table_import_ipc: frame %d describes %zu fields, the schema has %lld", f, L.nodes.size(),
+           (long long)n_fields);
+  FG_CHECK(L.length >= 0 && L.length < (int64_t(1) << 31), FLOCKGPU_ERR_INVALID, "table_import_ipc: frame %d: batch length %lld", f, (long long)L.length);
+  size_t next = 0;
+  for (int64_t c = 0; c < n_fields; ++c) {
+    const char* fmt = schema->children[c]->format;
+    const int dt = dtype_from_format(fmt);
+    FG_CHECK(dt >= 0, FLOCKGPU_ERR_UNSUPPORTED, "table_import_ipc: column \"%s\" has unsupported Arrow format \"%s\"", schema->children[c]->name, fmt ? fmt : "");
+    const size_t want = dt == FLOCKGPU_UTF8 ? 3 : 2;
+    FG_CHECK(next + want <= L.buffers.size(), FLOCKGPU_ERR_INVALID, "table_import_ipc: frame %d lists too few buffers", f);
+    const int64_t length = L.nodes[size_t(c)].first, null_count = L.nodes[size_t(c)].second;
+    FG_CHECK(length == L.length, FLOCKGPU_ERR_INVALID, "table_import_ipc: frame %d: field length %lld differs from the batch length %lld", f,
+             (long long)length, (long long)L.length);
+    FG_CHECK(null_count >= 0 && null_count <= length, FLOCKGPU_ERR_INVALID, "table_import_ipc: frame %d: null count %lld of %lld rows", f,
+             (long long)null_count, (long long)length);
+    for (size_t b = 0; b < want; ++b) {
+      const auto& ext = L.buffers[next + b];
+      FG_CHECK(ext.first >= 0 && ext.second >= 0 && ext.first <= body_len && ext.second <= body_len - ext.first, FLOCKGPU_ERR_INVALID,
+               "table_import_ipc: frame %d: buffer [%lld, +%lld) outside the %lld-byte body", f, (long long)ext.first, (long long)ext.second,
+               (long long)body_len);
+    }
+    // every buffer holds what `length` rows need (a frame that claims more rows than it carries would be read past its end)
+    const auto& validity = L.buffers[next];
+    FG_CHECK(validity.second == 0 ? null_count == 0 : validity.second >= (length + 7) / 8, FLOCKGPU_ERR_INVALID,
+             "table_import_ipc: frame %d, column \"%s\": validity bitmap of %lld bytes for %lld rows with %lld nulls", f, schema->children[c]->name,
+             (long long)validity.second, (long long)length, (long long)null_count);
+    if (dt == FLOCKGPU_UTF8) {
+      const auto& offs = L.buffers[next + 1];
+      FG_CHECK(length == 0 || offs.second >= (length + 1) * 4, FLOCKGPU_ERR_INVALID, "table_import_ipc: frame %d, column \"%s\": offsets buffer of %lld bytes for %lld rows", f,
+               schema->children[c]->name, (long long)offs.second, (long long)length);
+    } else {
+      const auto& data = L.buffers[next + 1];
+      FG_CHECK(data.second >= length * int64_t(dtype_width(dt)), FLOCKGPU_ERR_INVALID, "table_import_ipc: frame %d, column \"%s\": %lld value bytes for %lld rows", f,
+               schema->children[c]->name, (long long)data.second, (long long)length);
+    }
+    next += want;
+  }
+}
+
+void check_utf8_extent(int f, const char* column, int32_t first, int32_t last, int64_t value_bytes) {
+  FG_CHECK(first >= 0 && last >= first && int64_t(last) <= value_bytes, FLOCKGPU_ERR_INVALID, "table_import_ipc: frame %d, column \"%s\": offsets [%d, %d] outside the %lld value bytes", f,
+           column, first, last, (long long)value_bytes);
+}
+
 // Arrow C arrays whose buffers point INTO the frames' bodies: pure host work, no device, no context -- every offset and
 // length a frame claims is checked against the bytes it came with before anything dereferences them.
 struct IpcFrame {
@@ -158,58 +206,30 @@ IpcFrames view_ipc_frames(const ArrowSchema* schema, const uint8_t* const* heade
   for (int f = 0; f < n_frames; ++f) {
     FG_CHECK(body_lens[f] >= 0 && (body_lens[f] == 0 || bodies[f]), FLOCKGPU_ERR_INVALID, "table_import_ipc: frame %d has no body", f);
     const FrameLayout L = parse_record_batch_message(headers[f], header_lens[f]);
-    FG_CHECK(int64_t(L.nodes.size()) == n_fields, FLOCKGPU_ERR_INVALID, "table_import_ipc: frame %d describes %zu fields, the schema has %lld", f, L.nodes.size(),
-             (long long)n_fields);
-    FG_CHECK(L.length >= 0 && L.length < (int64_t(1) << 31), FLOCKGPU_ERR_INVALID, "table_import_ipc: frame %d: batch length %lld", f, (long long)L.length);
+    check_frame_layout(schema, f, L, body_lens[f]);
     auto fr = std::make_unique<IpcFrame>();
     fr->kids.resize(size_t(n_fields));
     fr->bufs.resize(size_t(n_fields));
     size_t next = 0;
     for (int64_t c = 0; c < n_fields; ++c) {
-      const char* fmt = schema->children[c]->format;
-      const int dt = dtype_from_format(fmt);
-      FG_CHECK(dt >= 0, FLOCKGPU_ERR_UNSUPPORTED, "table_import_ipc: column \"%s\" has unsupported Arrow format \"%s\"", schema->children[c]->name, fmt ? fmt : "");
+      const int dt = dtype_from_format(schema->children[c]->format);
       const size_t want = dt == FLOCKGPU_UTF8 ? 3 : 2;
-      FG_CHECK(next + want <= L.buffers.size(), FLOCKGPU_ERR_INVALID, "table_import_ipc: frame %d lists too few buffers", f);
       ArrowArray& a = fr->kids[size_t(c)];
       memset(&a, 0, sizeof a);
       a.length = L.nodes[size_t(c)].first;
       a.null_count = L.nodes[size_t(c)].second;
-      FG_CHECK(a.length == L.length, FLOCKGPU_ERR_INVALID, "table_import_ipc: frame %d: field length %lld differs from the batch length %lld", f,
-               (long long)a.length, (long long)L.length);
-      FG_CHECK(a.null_count >= 0 && a.null_count <= a.length, FLOCKGPU_ERR_INVALID, "table_import_ipc: frame %d: null count %lld of %lld rows", f,
-               (long long)a.null_count, (long long)a.length);
       for (size_t b = 0; b < want; ++b) {
         const auto& ext = L.buffers[next + b];
-        FG_CHECK(ext.first >= 0 && ext.second >= 0 && ext.first <= body_lens[f] && ext.second <= body_lens[f] - ext.first, FLOCKGPU_ERR_INVALID,
-                 "table_import_ipc: frame %d: buffer [%lld, +%lld) outside the %lld-byte body", f, (long long)ext.first, (long long)ext.second,
-                 (long long)body_lens[f]);
         // a zero-length validity buffer means "no nulls"; zero-length data buffers of empty batches still get an address
         const bool absent = ext.second == 0 && b == 0;
         fr->bufs[size_t(c)].push_back(absent ? nullptr : static_cast<const void*>(bodies[f] + ext.first));
       }
-      // every buffer holds what `length` rows need (a frame that claims more rows than it carries would be read past its end)
-      const auto& validity = L.buffers[next];
-      FG_CHECK(validity.second == 0 ? a.null_count == 0 : validity.second >= (a.length + 7) / 8, FLOCKGPU_ERR_INVALID,
-               "table_import_ipc: frame %d, column \"%s\": validity bitmap of %lld bytes for %lld rows with %lld nulls", f, schema->children[c]->name,
-               (long long)validity.second, (long long)a.length, (long long)a.null_count);
-      if (dt == FLOCKGPU_UTF8) {
+      if (dt == FLOCKGPU_UTF8 && a.length > 0) {
         const auto& offs = L.buffers[next + 1];
-        const auto& data = L.buffers[next + 2];
-        if (a.length > 0) {
-          FG_CHECK(offs.second >= (a.length + 1) * 4, FLOCKGPU_ERR_INVALID, "table_import_ipc: frame %d, column \"%s\": offsets buffer of %lld bytes for %lld rows", f,
-                   schema->children[c]->name, (long long)offs.second, (long long)a.length);
-          int32_t first, last;
-          memcpy(&first, bodies[f] + offs.first, 4);
-          memcpy(&last, bodies[f] + offs.first + a.length * 4, 4);
-          FG_CHECK(first >= 0 && last >= first && int64_t(last) <= data.second, FLOCKGPU_ERR_INVALID,
-                   "table_import_ipc: frame %d, column \"%s\": offsets [%d, %d] outside the %lld value bytes", f, schema->children[c]->name, first, last,
-                   (long long)data.second);
-        }
-      } else {
-        const auto& data = L.buffers[next + 1];
-        FG_CHECK(data.second >= a.length * int64_t(dtype_width(dt)), FLOCKGPU_ERR_INVALID, "table_import_ipc: frame %d, column \"%s\": %lld value bytes for %lld rows", f,
-                 schema->children[c]->name, (long long)data.second, (long long)a.length);
+        int32_t first, last;
+        memcpy(&first, bodies[f] + offs.first, 4);
+        memcpy(&last, bodies[f] + offs.first + a.length * 4, 4);
+        check_utf8_extent(f, schema->children[c]->name, first, last, L.buffers[next + 2].second);
       }
       next += want;
       a.n_buffers = int64_t(want);

@@ -411,6 +411,33 @@ using Expr = std::vector<ExprTok>;  // postfix
 
 TablePtr import_batches(const CtxPtr& ctx, const ArrowSchema* schema, const ArrowArray* const* batches,
                         int n_batches, const int* projection, int n_projection, bool zero_copy = false);
+// Host -> device copies, page-locked staging of pageable sources included (the copy path of import_batches); returns
+// once the copies have landed.
+struct HostPiece {
+  char* dst;
+  const char* src;
+  size_t bytes;
+  size_t stage_off;  // offset in the staging block: the pieces' running byte total
+};
+void upload_host_pieces(const CtxPtr& ctx, const std::vector<HostPiece>& pieces, size_t total_bytes);
+std::string copy_metadata(const char* md);  // the Arrow schema metadata block, verbatim
+
+// Arrow IPC record-batch messages (host/ipc.cc)
+struct FrameLayout {
+  int64_t length = 0;
+  int64_t body_length = -1;                          // Message.bodyLength (-1: absent)
+  std::vector<std::pair<int64_t, int64_t>> nodes;    // (length, null_count) per field
+  std::vector<std::pair<int64_t, int64_t>> buffers;  // (offset, length) into the body
+};
+FrameLayout parse_record_batch_message(const uint8_t* header, int64_t header_len);
+void check_frame_layout(const ArrowSchema* schema, int f, const FrameLayout& L, int64_t body_len);
+void check_utf8_extent(int f, const char* column, int32_t first, int32_t last, int64_t value_bytes);
+
+// zstd payload frames (zstd.cu).  zstd_decode_host: every frame of src[0, n) serially on the host (headers, self test);
+// returns a zstd::Z_* code, 0 on success.
+int zstd_decode_host(const uint8_t* src, int64_t n, int64_t max_out, std::vector<uint8_t>* out);
+TablePtr import_payload_zstd(flockgpu_ctx* ctx, const ArrowSchema* schema, const uint8_t* const* headers, const int64_t* header_lens,
+                             const uint8_t* const* bodies, const int64_t* body_lens, int n_frames, const int* projection, int n_projection);
 void export_table(const CtxPtr& ctx, const Table& t, int64_t row_begin, int64_t row_count,
                   ArrowSchema* out_schema, ArrowArray* out_array);
 void export_schema(const Table& t, ArrowSchema* out_schema);

@@ -7,6 +7,7 @@
 #include "expr_compile.h"
 #include "internal.h"
 #include "pred_i32.h"
+#include "zstd_dec.h"
 
 using namespace fg;
 
@@ -118,3 +119,16 @@ int flockgpu_selftest_pred_i32(int64_t modulus, int32_t cmp, int64_t rhs, const 
   });
 }
 
+// The zstd decoder of the payload import (zstd_dec.h) run serially on the host: what CPU CI compares byte for byte with
+// another implementation.
+int flockgpu_selftest_zstd_decompress(const uint8_t* src, int64_t src_len, uint8_t* dst, int64_t capacity, int64_t* out_len) {
+  return guarded([&] {
+    FG_CHECK(src_len >= 0 && (src || src_len == 0) && capacity >= 0 && (dst || capacity == 0) && out_len, FLOCKGPU_ERR_INVALID,
+             "selftest_zstd_decompress: bad arguments");
+    std::vector<uint8_t> out;
+    const int e = zstd_decode_host(src, src_len, capacity, &out);
+    FG_CHECK(!e, e == zstd::Z_DICTIONARY ? FLOCKGPU_ERR_UNSUPPORTED : FLOCKGPU_ERR_INVALID, "selftest_zstd_decompress: %s", zstd::error_name(e));
+    if (!out.empty()) memcpy(dst, out.data(), out.size());
+    *out_len = int64_t(out.size());
+  });
+}

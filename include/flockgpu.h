@@ -155,6 +155,23 @@ int flockgpu_table_export(flockgpu_ctx* ctx, const flockgpu_table* table, int64_
 int flockgpu_table_import_ipc(flockgpu_ctx* ctx, const struct ArrowSchema* schema, const uint8_t* const* headers, const int64_t* header_lens,
                               const uint8_t* const* bodies, const int64_t* body_lens, int32_t n_frames, const int32_t* projection,
                               int32_t n_projection, flockgpu_table** out);
+/* Host -> HBM from a payload's DataFrames as they arrive, compressed with the payload's encoding (flock/src/runtime/
+ * payload.rs:161-192 Payload::to_record_batch decompresses every frame with libzstd on the CPU, flock/src/transmute.rs:
+ * 178-221 to_payload compresses them with zstd::block::compress(.., 3); the codecs: flock/src/encoding.rs).
+ * `encoding` is Flock's `Encoding` discriminant (FLOCKGPU_ENCODING_*).  `header_lens` / `body_lens` are the COMPRESSED
+ * lengths.  NONE is flockgpu_table_import_ipc.  ZSTD: the ~100-byte headers are decoded on the host, the bodies are copied
+ * to HBM compressed and decoded there (RFC 8878; concatenated and skippable frames are accepted, Content_Checksum is not
+ * verified, a Dictionary_ID other than 0 is FLOCKGPU_ERR_UNSUPPORTED); every body must decode to exactly its header's
+ * bodyLength.  A malformed frame is FLOCKGPU_ERR_INVALID naming it, and the context stays usable.  SNAPPY, LZ4 and ZLIB:
+ * FLOCKGPU_ERR_UNSUPPORTED (the caller decompresses those itself); any other value: FLOCKGPU_ERR_INVALID.              */
+#define FLOCKGPU_ENCODING_SNAPPY 0
+#define FLOCKGPU_ENCODING_LZ4 1
+#define FLOCKGPU_ENCODING_ZLIB 2
+#define FLOCKGPU_ENCODING_ZSTD 3
+#define FLOCKGPU_ENCODING_NONE 4
+int flockgpu_table_import_payload(flockgpu_ctx* ctx, const struct ArrowSchema* schema, int32_t encoding, const uint8_t* const* headers,
+                                  const int64_t* header_lens, const uint8_t* const* bodies, const int64_t* body_lens, int32_t n_frames,
+                                  const int32_t* projection, int32_t n_projection, flockgpu_table** out);
 /* HBM -> one DataFrame for rows [row_begin, row_begin + row_count) (row_count < 0: to the end): *out_header receives a
  * flatbuffer Message { RecordBatch } (MetadataVersion V5, 8-byte aligned buffers, what arrow-rs writes), *out_body the
  * buffers.  Both blocks belong to the caller and are released with flockgpu_ipc_free.                                */
@@ -373,6 +390,10 @@ int flockgpu_selftest_eval_value(const struct ArrowSchema* schema, const struct 
 /* CPU-only: the arithmetic of the vectorised filter predicate CAST(x AS Int64) [% modulus] cmp rhs (modulus 0 = no `%`),
  * with the constants and the per-row test the GPU kernel uses (flock_b200/csrc/pred_i32.h).  out_keep[i] in {0, 1}. */
 int flockgpu_selftest_pred_i32(int64_t modulus, int32_t cmp, int64_t rhs, const int32_t* x, int64_t n, uint8_t* out_keep, int32_t* out_mode);
+/* CPU-only: decodes a zstd stream (RFC 8878; every frame of src, skippable frames skipped) with the decoder functions the
+ * payload-import kernels use (flock_b200/csrc/zstd_dec.h), serially on the host.  *out_len = decoded bytes; more than
+ * `capacity` is FLOCKGPU_ERR_INVALID, as is any malformed input.                                                         */
+int flockgpu_selftest_zstd_decompress(const uint8_t* src, int64_t src_len, uint8_t* dst, int64_t capacity, int64_t* out_len);
 
 #ifdef __cplusplus
 }

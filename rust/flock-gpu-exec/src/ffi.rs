@@ -53,6 +53,22 @@ extern "C" {
         n_projection: i32,
         out: *mut *mut flockgpu_table,
     ) -> c_int;
+    /// Payload frames as they arrive, compressed with `encoding` (Flock's `Encoding` discriminant, `payload.encoding as
+    /// i32`): Zstd bodies are decoded on the GPU, None is flockgpu_table_import_ipc, Snappy / Lz4 / Zlib return
+    /// FLOCKGPU_ERR_UNSUPPORTED.  header_lens / body_lens are the compressed lengths.
+    pub fn flockgpu_table_import_payload(
+        ctx: *mut flockgpu_ctx,
+        schema: *const FFI_ArrowSchema,
+        encoding: i32,
+        headers: *const *const u8,
+        header_lens: *const i64,
+        bodies: *const *const u8,
+        body_lens: *const i64,
+        n_frames: i32,
+        projection: *const i32,
+        n_projection: i32,
+        out: *mut *mut flockgpu_table,
+    ) -> c_int;
     pub fn flockgpu_table_export_ipc(
         ctx: *mut flockgpu_ctx,
         table: *const flockgpu_table,

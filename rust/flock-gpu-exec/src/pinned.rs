@@ -7,7 +7,8 @@
 //! that create the batches a worker function executes on are `Payload::to_record_batch` (flock/src/runtime/
 //! payload.rs:161-192) and `Arena::take` (flock/src/runtime/arena/mod.rs:114-169): both decode (and, with
 //! Encoding::Zstd, decompress) into freshly allocated memory anyway, so decoding INTO page-locked memory costs
-//! nothing extra -- `pinned_batch` below is the copy form for batches that already exist.
+//! nothing extra -- `pinned_batch` below is the copy form for batches that already exist.  `frames_to_table` skips
+//! host batches altogether: zstd frames are decompressed on the GPU.
 //!
 //! SOURCE ONLY (no cargo / rustc in the build image): never compiled.
 use crate::ffi;
@@ -108,12 +109,16 @@ pub fn pinned_batch(ctx: *mut ffi::flockgpu_ctx, batch: &RecordBatch) -> ArrowRe
     RecordBatch::try_new(batch.schema(), columns)
 }
 
-/// `Payload::to_record_batch` for Encoding::None frames WITHOUT going through host record batches at all: the frames
-/// go straight to a device table (flockgpu_table_import_ipc), which `flock_context_feed_tables` hands to the plan.
+/// `Payload::to_record_batch` WITHOUT going through host record batches at all: the frames go straight to a device
+/// table (flockgpu_table_import_payload), which `flock_context_feed_tables` hands to the plan.  `encoding` is the
+/// payload's `Encoding` (`payload.encoding as i32`): Zstd frames (Flock's default) are decompressed on the GPU, so the
+/// CPU decompress is gone; None frames are imported as they are.  `None` back (FLOCKGPU_ERR_UNSUPPORTED for Snappy /
+/// Lz4 / Zlib, or any error): the caller keeps its CPU route for this payload.
 pub fn frames_to_table(
     ctx: *mut ffi::flockgpu_ctx,
     schema: &FFI_ArrowSchema,
-    frames: &[(Vec<u8>, Vec<u8>)], // DataFrame { header, body }
+    encoding: i32,
+    frames: &[(Vec<u8>, Vec<u8>)], // DataFrame { header, body }, as they arrived (compressed with `encoding`)
 ) -> Option<*mut ffi::flockgpu_table> {
     let headers: Vec<*const u8> = frames.iter().map(|f| f.0.as_ptr()).collect();
     let header_lens: Vec<i64> = frames.iter().map(|f| f.0.len() as i64).collect();
@@ -121,9 +126,10 @@ pub fn frames_to_table(
     let body_lens: Vec<i64> = frames.iter().map(|f| f.1.len() as i64).collect();
     let mut out = std::ptr::null_mut();
     let rc = unsafe {
-        ffi::flockgpu_table_import_ipc(
+        ffi::flockgpu_table_import_payload(
             ctx,
             schema,
+            encoding,
             headers.as_ptr(),
             header_lens.as_ptr(),
             bodies.as_ptr(),
