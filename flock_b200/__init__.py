@@ -218,6 +218,27 @@ class Table:
             lib.flockgpu_ipc_free(h)
             lib.flockgpu_ipc_free(b)
 
+    def to_payload(self, encoding: str = "zstd", rows_per_frame: int = 65536) -> list[tuple[bytes, bytes]]:
+        """The payload's DataFrames as (header, body) pairs, frame f = rows [f * rows_per_frame, (f + 1) * rows_per_frame):
+        the reference's `to_payload`.  "zstd" (its default) compresses every body on the GPU and every header on the host,
+        each as one zstd frame; "none" gives what `to_ipc` gives for each row range.  A zstd body over 10 MiB raises
+        FlockGpuError(ERR_INVALID) naming the frame; "snappy" / "lz4" / "zlib" raise FlockGpuError(ERR_UNSUPPORTED)."""
+        code = ENCODINGS.get(encoding, encoding) if isinstance(encoding, str) else int(encoding)
+        if isinstance(code, str):
+            raise ValueError(f"unknown encoding {encoding!r}; one of {sorted(ENCODINGS)}")
+        p = C.c_void_p()
+        check(lib.flockgpu_table_export_payload(self.ctx.handle, self.handle, code, rows_per_frame, C.byref(p)))
+        try:
+            out = []
+            h, b = C.c_void_p(), C.c_void_p()
+            hl, bl = C.c_int64(), C.c_int64()
+            for i in range(lib.flockgpu_payload_num_frames(p)):
+                check(lib.flockgpu_payload_frame(p, i, C.byref(h), C.byref(hl), C.byref(b), C.byref(bl)))
+                out.append((C.string_at(h, hl.value), C.string_at(b, bl.value)))
+            return out
+        finally:
+            lib.flockgpu_payload_free(p)
+
     def release(self) -> None:
         if self.handle:
             lib.flockgpu_table_release(self.handle)
@@ -535,6 +556,17 @@ def selftest_zstd_decompress(data: bytes, capacity: int) -> bytes:
     dst = C.create_string_buffer(max(capacity, 1))
     n = C.c_int64()
     check(lib.flockgpu_selftest_zstd_decompress(C.c_void_p(src.address), src.size, dst, capacity, C.byref(n)))
+    return dst.raw[:n.value]
+
+
+def selftest_zstd_compress(data: bytes) -> bytes:
+    """CPU-only: one zstd frame of `data` from the encoder functions of the GPU payload export (csrc/zstd_enc.h), run
+    serially on the host: byte for byte what `Table.to_payload("zstd")` gives for the same body."""
+    src = pa.py_buffer(data)
+    capacity = 32 + src.size + 3 * (src.size // (128 << 10) + 1)
+    dst = C.create_string_buffer(capacity)
+    n = C.c_int64()
+    check(lib.flockgpu_selftest_zstd_compress(C.c_void_p(src.address), src.size, dst, capacity, C.byref(n)))
     return dst.raw[:n.value]
 
 

@@ -130,6 +130,10 @@ PROTOTYPES = {
                                                C.POINTER(C.c_int64), C.c_int32, _I32P, C.c_int32, _PP]),
     "flockgpu_table_export_ipc": (C.c_int, [_P, _P, C.c_int64, C.c_int64, _PP, C.POINTER(C.c_int64), _PP, C.POINTER(C.c_int64)]),
     "flockgpu_ipc_free": (None, [_P]),
+    "flockgpu_table_export_payload": (C.c_int, [_P, _P, C.c_int32, C.c_int64, _PP]),
+    "flockgpu_payload_num_frames": (C.c_int32, [_P]),
+    "flockgpu_payload_frame": (C.c_int, [_P, C.c_int32, _PP, C.POINTER(C.c_int64), _PP, C.POINTER(C.c_int64)]),
+    "flockgpu_payload_free": (None, [_P]),
     "flockgpu_table_import_ndjson": (C.c_int, [_P, C.POINTER(ArrowSchema), _P, C.c_int64, _PP]),
     "flockgpu_table_retain": (C.c_int, [_P]),
     "flockgpu_table_release": (C.c_int, [_P]),
@@ -167,6 +171,7 @@ PROTOTYPES = {
     "flockgpu_selftest_eval_predicate": (C.c_int, [C.POINTER(ArrowSchema), C.POINTER(ArrowArray), C.POINTER(Expr), _P, _I32P]),
     "flockgpu_selftest_eval_value": (C.c_int, [C.POINTER(ArrowSchema), C.POINTER(ArrowArray), C.POINTER(Expr), _P, _I32P, _I32P]),
     "flockgpu_selftest_zstd_decompress": (C.c_int, [_P, C.c_int64, _P, C.c_int64, C.POINTER(C.c_int64)]),
+    "flockgpu_selftest_zstd_compress": (C.c_int, [_P, C.c_int64, _P, C.c_int64, C.POINTER(C.c_int64)]),
     "flockgpu_selftest_pred_i32": (C.c_int, [C.c_int64, C.c_int32, C.c_int64, _I32P, C.c_int64, C.POINTER(C.c_uint8), _I32P]),
 }
 

@@ -11,8 +11,9 @@
 // extents, the extents become Arrow C arrays that point INTO the bodies, and the ordinary import (core.cu:
 // import_batches) moves them to HBM (projection pushdown, staging of pageable memory and the zero-copy feed of
 // page-locked bodies included).  Export: the inverse; the body is filled by device-to-host copies straight into its
-// final place and the flatbuffer header is written by hand.  Encoding::None only: the reference's zstd / lz4 / snappy
-// block codecs (flock/src/encoding.rs:59-99) sit in front of this and are not restated (DESIGN.md section 7).
+// final place and the flatbuffer header is written by hand.  Encoding::None only: zstd frames are decoded by zstd.cu
+// and encoded by zstd_enc.cu (which reuses build_record_batch_message); lz4 / snappy / zlib are not restated
+// (DESIGN.md section 7).
 #include <cstring>
 #include <memory>
 #include <vector>
@@ -87,6 +88,8 @@ struct Out {
   }
 };
 
+}  // namespace
+
 std::vector<uint8_t> build_record_batch_message(int64_t length, const std::vector<std::pair<int64_t, int64_t>>& nodes,
                                                 const std::vector<std::pair<int64_t, int64_t>>& buffers, int64_t body_len) {
   // fixed layout, every offset pointing forward:
@@ -131,8 +134,6 @@ std::vector<uint8_t> build_record_batch_message(int64_t length, const std::vecto
   o.b.resize((o.b.size() + 7) & ~size_t(7), 0);
   return o.b;
 }
-
-}  // namespace
 
 // Everything about frame `f` that its header alone decides, against the schema and a body of `body_len` bytes: field
 // count, batch and field lengths, null counts, and every buffer extent.  The Utf8 offsets live in the body; the caller

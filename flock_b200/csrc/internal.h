@@ -432,10 +432,15 @@ struct FrameLayout {
 FrameLayout parse_record_batch_message(const uint8_t* header, int64_t header_len);
 void check_frame_layout(const ArrowSchema* schema, int f, const FrameLayout& L, int64_t body_len);
 void check_utf8_extent(int f, const char* column, int32_t first, int32_t last, int64_t value_bytes);
+// The flatbuffer Message { RecordBatch } of one frame: (length, null_count) per field, (offset, length) per buffer.
+std::vector<uint8_t> build_record_batch_message(int64_t length, const std::vector<std::pair<int64_t, int64_t>>& nodes,
+                                                const std::vector<std::pair<int64_t, int64_t>>& buffers, int64_t body_len);
 
 // zstd payload frames (zstd.cu).  zstd_decode_host: every frame of src[0, n) serially on the host (headers, self test);
 // returns a zstd::Z_* code, 0 on success.
 int zstd_decode_host(const uint8_t* src, int64_t n, int64_t max_out, std::vector<uint8_t>* out);
+// One zstd frame of src[0, n) appended to *out, by the export kernel's encoder phases run serially (zstd_enc.cu).
+void zstd_compress_host(const uint8_t* src, int64_t n, std::vector<uint8_t>* out);
 TablePtr import_payload_zstd(flockgpu_ctx* ctx, const ArrowSchema* schema, const uint8_t* const* headers, const int64_t* header_lens,
                              const uint8_t* const* bodies, const int64_t* body_lens, int n_frames, const int* projection, int n_projection);
 void export_table(const CtxPtr& ctx, const Table& t, int64_t row_begin, int64_t row_count,

@@ -132,3 +132,17 @@ int flockgpu_selftest_zstd_decompress(const uint8_t* src, int64_t src_len, uint8
     *out_len = int64_t(out.size());
   });
 }
+
+// The zstd encoder of the payload export (zstd_enc.h) run serially on the host: the bytes the GPU gives for the same
+// input, which CPU CI decompresses with another implementation.
+int flockgpu_selftest_zstd_compress(const uint8_t* src, int64_t src_len, uint8_t* dst, int64_t capacity, int64_t* out_len) {
+  return guarded([&] {
+    FG_CHECK(src_len >= 0 && (src || src_len == 0) && capacity >= 0 && (dst || capacity == 0) && out_len, FLOCKGPU_ERR_INVALID,
+             "selftest_zstd_compress: bad arguments");
+    std::vector<uint8_t> out;
+    zstd_compress_host(src, src_len, &out);
+    FG_CHECK(int64_t(out.size()) <= capacity, FLOCKGPU_ERR_INVALID, "selftest_zstd_compress: %zu compressed bytes, capacity %lld", out.size(), (long long)capacity);
+    memcpy(dst, out.data(), out.size());
+    *out_len = int64_t(out.size());
+  });
+}

@@ -178,6 +178,24 @@ int flockgpu_table_import_payload(flockgpu_ctx* ctx, const struct ArrowSchema* s
 int flockgpu_table_export_ipc(flockgpu_ctx* ctx, const flockgpu_table* table, int64_t row_begin, int64_t row_count, uint8_t** out_header,
                               int64_t* out_header_len, uint8_t** out_body, int64_t* out_body_len);
 void flockgpu_ipc_free(uint8_t* block);
+/* HBM -> the DataFrames of a payload (flock/src/transmute.rs:178-221 to_payload).  Frame f holds rows
+ * [f * rows_per_frame, min((f + 1) * rows_per_frame, rows)); a table of 0 rows gives 0 frames.  Each frame's
+ * uncompressed header and body are exactly what flockgpu_table_export_ipc returns for that row range.
+ * encoding NONE: those bytes.  ZSTD: each header and each body compressed as one zstd frame (RFC 8878; Single_Segment,
+ * Frame_Content_Size = the uncompressed length, no checksum, no dictionary); bodies are packed and compressed on the
+ * GPU and only the compressed bytes cross the link, headers are compressed on the host.  A body larger than
+ * 10 MiB (what Flock's receiver decompresses into, flock/src/encoding.rs:92) is FLOCKGPU_ERR_INVALID naming the frame
+ * under ZSTD.  SNAPPY / LZ4 / ZLIB: FLOCKGPU_ERR_UNSUPPORTED; any other encoding, or rows_per_frame <= 0:
+ * FLOCKGPU_ERR_INVALID.  The same table gives the same bytes on every call.  *out owns every frame's bytes (the bodies
+ * in page-locked memory) until flockgpu_payload_free.                                                               */
+typedef struct flockgpu_payload flockgpu_payload;
+int flockgpu_table_export_payload(flockgpu_ctx* ctx, const flockgpu_table* table, int32_t encoding, int64_t rows_per_frame,
+                                  flockgpu_payload** out);
+int32_t flockgpu_payload_num_frames(const flockgpu_payload* p);
+/* Frame i's header and body; the pointers stay valid until flockgpu_payload_free.                                      */
+int flockgpu_payload_frame(const flockgpu_payload* p, int32_t i, const uint8_t** header, int64_t* header_len, const uint8_t** body,
+                           int64_t* body_len);
+void flockgpu_payload_free(flockgpu_payload* p);
 /* ---- NDJSON events -> table: event_bytes_to_batch (flock/src/transmute.rs:255-266; call sites flock/src/datasource/
  *      nexmark/nexmark.rs:181-203), the schema-driven arrow json::Reader over the generator's serde_json lines ---------
  * One flat JSON object per line; fields are matched BY NAME in any order, unknown fields (nested values included) are
@@ -394,6 +412,10 @@ int flockgpu_selftest_pred_i32(int64_t modulus, int32_t cmp, int64_t rhs, const 
  * payload-import kernels use (flock_b200/csrc/zstd_dec.h), serially on the host.  *out_len = decoded bytes; more than
  * `capacity` is FLOCKGPU_ERR_INVALID, as is any malformed input.                                                         */
 int flockgpu_selftest_zstd_decompress(const uint8_t* src, int64_t src_len, uint8_t* dst, int64_t capacity, int64_t* out_len);
+/* CPU-only: compresses src into one zstd frame with the encoder functions the payload-export kernel uses
+ * (flock_b200/csrc/zstd_enc.h), serially on the host: byte for byte what flockgpu_table_export_payload(ZSTD) gives for
+ * the same body.  *out_len = compressed bytes; more than `capacity` is FLOCKGPU_ERR_INVALID.                          */
+int flockgpu_selftest_zstd_compress(const uint8_t* src, int64_t src_len, uint8_t* dst, int64_t capacity, int64_t* out_len);
 
 #ifdef __cplusplus
 }

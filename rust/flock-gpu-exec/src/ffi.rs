@@ -14,11 +14,16 @@ pub struct flockgpu_table {
     _private: [u8; 0],
 }
 #[repr(C)]
+pub struct flockgpu_payload {
+    _private: [u8; 0],
+}
+#[repr(C)]
 pub struct flock_context {
     _private: [u8; 0],
 }
 
 pub const FLOCKGPU_OK: c_int = 0;
+pub const FLOCKGPU_ERR_INVALID: c_int = -1;
 pub const FLOCKGPU_ERR_UNSUPPORTED: c_int = -2;
 
 extern "C" {
@@ -80,8 +85,27 @@ extern "C" {
         out_body_len: *mut i64,
     ) -> c_int;
     pub fn flockgpu_ipc_free(block: *mut u8);
+    /// HBM -> a payload's DataFrames, rows_per_frame rows each; ZSTD bodies are compressed on the GPU.
+    pub fn flockgpu_table_export_payload(
+        ctx: *mut flockgpu_ctx,
+        table: *const flockgpu_table,
+        encoding: i32,
+        rows_per_frame: i64,
+        out: *mut *mut flockgpu_payload,
+    ) -> c_int;
+    pub fn flockgpu_payload_num_frames(p: *const flockgpu_payload) -> i32;
+    pub fn flockgpu_payload_frame(
+        p: *const flockgpu_payload,
+        i: i32,
+        header: *mut *const u8,
+        header_len: *mut i64,
+        body: *mut *const u8,
+        body_len: *mut i64,
+    ) -> c_int;
+    pub fn flockgpu_payload_free(p: *mut flockgpu_payload);
     pub fn flock_context_feed_tables(ec: *mut flock_context, tables: *const *mut flockgpu_table, n_sources: i32) -> c_int;
     pub fn flockgpu_table_num_rows(table: *const flockgpu_table) -> i64;
+    pub fn flockgpu_table_nbytes(table: *const flockgpu_table) -> i64;
 
     // flock::runtime::context::ExecutionContext on the GPU
     pub fn flock_context_unmarshal(ctx: *mut flockgpu_ctx, plans_json: *const c_char, out: *mut *mut flock_context) -> c_int;

@@ -8,7 +8,8 @@
 //! payload.rs:161-192) and `Arena::take` (flock/src/runtime/arena/mod.rs:114-169): both decode (and, with
 //! Encoding::Zstd, decompress) into freshly allocated memory anyway, so decoding INTO page-locked memory costs
 //! nothing extra -- `pinned_batch` below is the copy form for batches that already exist.  `frames_to_table` skips
-//! host batches altogether: zstd frames are decompressed on the GPU.
+//! host batches altogether: zstd frames are decompressed on the GPU; `table_to_frames` is its inverse, compressing on
+//! the GPU.
 //!
 //! SOURCE ONLY (no cargo / rustc in the build image): never compiled.
 use crate::ffi;
@@ -144,6 +145,47 @@ pub fn frames_to_table(
         Some(out)
     } else {
         None
+    }
+}
+
+/// `to_payload` (flock/src/transmute.rs:178-221) WITHOUT host record batches: the device table becomes the payload's
+/// DataFrames { header, body } (flockgpu_table_export_payload); with Encoding::Zstd (`encoding = 3`, Flock's default)
+/// the bodies are compressed on the GPU and only compressed bytes cross the link.  `rows_per_frame: None` picks a frame
+/// size whose body stays within the 10 MiB Flock's receiver decompresses into (flock/src/encoding.rs:92): at most
+/// 65,536 rows and about 8 MiB of the table's bytes per frame, halved while a frame is still too large.  `None` back
+/// (FLOCKGPU_ERR_UNSUPPORTED for Snappy / Lz4 / Zlib, or any other error): the caller keeps its CPU route.
+pub fn table_to_frames(
+    ctx: *mut ffi::flockgpu_ctx,
+    table: *const ffi::flockgpu_table,
+    encoding: i32,
+    rows_per_frame: Option<i64>,
+) -> Option<Vec<(Vec<u8>, Vec<u8>)>> {
+    let rows = unsafe { ffi::flockgpu_table_num_rows(table) }.max(1);
+    let bytes = unsafe { ffi::flockgpu_table_nbytes(table) }.max(1);
+    let mut rpf = rows_per_frame.unwrap_or_else(|| ((8i64 << 20) as i128 * rows as i128 / bytes as i128).clamp(1, 65536) as i64);
+    loop {
+        let mut p = std::ptr::null_mut();
+        let rc = unsafe { ffi::flockgpu_table_export_payload(ctx, table, encoding, rpf, &mut p) };
+        if rc == ffi::FLOCKGPU_ERR_INVALID && rows_per_frame.is_none() && rpf > 1 {
+            rpf /= 2; // a frame's body is over 10 MiB: smaller frames
+            continue;
+        }
+        if rc != ffi::FLOCKGPU_OK {
+            return None;
+        }
+        let n = unsafe { ffi::flockgpu_payload_num_frames(p) };
+        let mut frames = Vec::with_capacity(n as usize);
+        for i in 0..n {
+            let (mut h, mut hl, mut b, mut bl) = (std::ptr::null(), 0i64, std::ptr::null(), 0i64);
+            if unsafe { ffi::flockgpu_payload_frame(p, i, &mut h, &mut hl, &mut b, &mut bl) } != ffi::FLOCKGPU_OK {
+                unsafe { ffi::flockgpu_payload_free(p) };
+                return None;
+            }
+            let copy = |ptr: *const u8, len: i64| if len == 0 { vec![] } else { unsafe { std::slice::from_raw_parts(ptr, len as usize) }.to_vec() };
+            frames.push((copy(h, hl), copy(b, bl)));
+        }
+        unsafe { ffi::flockgpu_payload_free(p) };
+        return Some(frames);
     }
 }
 
