@@ -430,11 +430,39 @@ struct FrameLayout {
   std::vector<std::pair<int64_t, int64_t>> buffers;  // (offset, length) into the body
 };
 FrameLayout parse_record_batch_message(const uint8_t* header, int64_t header_len);
+// Index of each field's first buffer in FrameLayout::buffers (Utf8: validity, offsets, values; every other type:
+// validity, values); the last entry is the buffer count.
+std::vector<size_t> field_buffers(const ArrowSchema* schema);
 void check_frame_layout(const ArrowSchema* schema, int f, const FrameLayout& L, int64_t body_len);
 void check_utf8_extent(int f, const char* column, int32_t first, int32_t last, int64_t value_bytes);
-// The flatbuffer Message { RecordBatch } of one frame: (length, null_count) per field, (offset, length) per buffer.
-std::vector<uint8_t> build_record_batch_message(int64_t length, const std::vector<std::pair<int64_t, int64_t>>& nodes,
-                                                const std::vector<std::pair<int64_t, int64_t>>& buffers, int64_t body_len);
+
+// The bodies of frames of `t` (dense), one per (first row, row count), laid out and packed on the device:
+// payload_layout_kernel reads the Utf8 extents and null counts (one small read-back, none when every range is empty),
+// then one segment launch writes every body.  Each body is exactly what an Arrow IPC writer gives for its rows.
+struct PackedFrames {
+  BufferPtr bodies;                           // every frame's body in HBM, 16-byte aligned, back to back, zero padding
+  std::vector<int64_t> body_at, body_len;
+  std::vector<std::vector<uint8_t>> headers;  // the uncompressed Message { RecordBatch } of each frame
+};
+PackedFrames pack_frames(const CtxPtr& ctx, const Table& t, const std::vector<std::pair<int64_t, int64_t>>& row_ranges);
+
+// One CTA's piece of ipc_segment_kernel, which moves bytes between IPC bodies and column buffers (import assemble,
+// export pack).  kCopy: n bytes; kOffsets: n int32 words, each + arg (the source may be unaligned); kBitsToBytes:
+// n validity bits -> n bytes; kBytesToBits: n validity bytes -> ceil(n / 8) bitmap bytes; kFill: n bytes = arg;
+// kSetI32: one int32 = arg.
+struct Seg {
+  enum Kind : int32_t { kCopy, kOffsets, kBitsToBytes, kBytesToBits, kFill, kSetI32 };
+  const uint8_t* src;
+  uint8_t* dst;
+  int64_t n;
+  int32_t kind, arg;
+};
+// Appends the segments of n elements (bytes, words or rows), cut into pieces of at most 64 KiB.
+void add_segs(std::vector<Seg>& segs, int kind, const uint8_t* src, uint8_t* dst, int64_t n, int32_t arg = 0);
+// Uploads `segs` and runs them: exactly one launch, even for an empty list.  The launch is profiled under `stage`
+// ("payload_assemble_kernel" at import, "payload_pack_kernel" at export), so a profile that spans an export and an
+// import keeps the two apart.
+void launch_segments(const CtxPtr& ctx, const std::vector<Seg>& segs, const char* stage);
 
 // zstd payload frames (zstd.cu).  zstd_decode_host: every frame of src[0, n) serially on the host (headers, self test);
 // returns a zstd::Z_* code, 0 on success.

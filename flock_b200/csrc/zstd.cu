@@ -15,7 +15,8 @@
 //                                     streams, the LL / OF / ML tables, the sequences -> (ll, ml, offset value).
 //             zstd_execute_kernel     one warp per body: blocks in order, repeat offsets resolved in frame order,
 //                                     literals and matches copied into the decoded body (DESIGN.md section 3, K11).
-//             payload_assemble_kernel one launch over a segment list: the projected columns from the decoded bodies.
+//             ipc_segment_kernel      one launch over a segment list: the projected columns from the decoded bodies
+//                                     (host/ipc.cc, shared with the export's pack; profiled as payload_assemble_kernel).
 //   A fixed number of launches per import, whatever the number of frames.  Errors found on the device are recorded
 //   per body (first one wins) and read back with the sync the import performs anyway: FLOCKGPU_ERR_INVALID naming
 //   the frame, never a fault.
@@ -173,15 +174,6 @@ struct ZBody {
   int64_t out, len;  // decoded body in the decoded scratch, its bodyLength
   int32_t first_block, n_blocks;
   int32_t ext_first, ext_n;  // Utf8 offset words to read back once decoded
-};
-
-// One assemble segment.  kind 0: copy n bytes; 1: n Utf8 offsets, each + arg; 2: n validity bits -> bytes;
-// 3: n bytes = arg; 4: one int32 = arg.
-struct Seg {
-  const uint8_t* src;
-  uint8_t* dst;
-  int64_t n;
-  int32_t kind, arg;
 };
 
 constexpr unsigned kFull = 0xFFFFFFFFu;
@@ -400,47 +392,6 @@ __global__ void __launch_bounds__(32) zstd_execute_kernel(const uint8_t* __restr
   }
 }
 
-// ---- payload_assemble_kernel: one CTA per segment ----------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) payload_assemble_kernel(const Seg* __restrict__ segs, int n_segs) {
-  for (int s = blockIdx.x; s < n_segs; s += gridDim.x) {
-    const Seg g = segs[s];
-    const int64_t n = g.n;
-    switch (g.kind) {
-      case 0: {
-        const uintptr_t a = reinterpret_cast<uintptr_t>(g.src) | reinterpret_cast<uintptr_t>(g.dst) | uintptr_t(n);
-        if ((a & 15) == 0) {
-          for (int64_t k = threadIdx.x; k < n / 16; k += blockDim.x) reinterpret_cast<uint4*>(g.dst)[k] = reinterpret_cast<const uint4*>(g.src)[k];
-        } else if ((a & 3) == 0) {
-          for (int64_t k = threadIdx.x; k < n / 4; k += blockDim.x) reinterpret_cast<uint32_t*>(g.dst)[k] = reinterpret_cast<const uint32_t*>(g.src)[k];
-        } else {
-          for (int64_t k = threadIdx.x; k < n; k += blockDim.x) g.dst[k] = g.src[k];
-        }
-        break;
-      }
-      case 1: {
-        int32_t* d = reinterpret_cast<int32_t*>(g.dst);
-        if ((reinterpret_cast<uintptr_t>(g.src) & 3) == 0) {
-          for (int64_t r = threadIdx.x; r < n; r += blockDim.x) d[r] = reinterpret_cast<const int32_t*>(g.src)[r] + g.arg;
-        } else {
-          for (int64_t r = threadIdx.x; r < n; r += blockDim.x) {
-            const uint8_t* w = g.src + 4 * r;
-            d[r] = int32_t(uint32_t(w[0]) | (uint32_t(w[1]) << 8) | (uint32_t(w[2]) << 16) | (uint32_t(w[3]) << 24)) + g.arg;
-          }
-        }
-        break;
-      }
-      case 2:
-        for (int64_t r = threadIdx.x; r < n; r += blockDim.x) g.dst[r] = (g.src[r >> 3] >> (r & 7)) & 1;
-        break;
-      case 3:
-        for (int64_t r = threadIdx.x; r < n; r += blockDim.x) g.dst[r] = uint8_t(g.arg);
-        break;
-      default:
-        if (threadIdx.x == 0) *reinterpret_cast<int32_t*>(g.dst) = g.arg;
-    }
-  }
-}
-
 // ---- host orchestration ------------------------------------------------------------------------------------------------------
 [[noreturn]] void body_error(int f, int code, int64_t at) {
   fail(code == zs::Z_DICTIONARY ? FLOCKGPU_ERR_UNSUPPORTED : FLOCKGPU_ERR_INVALID, "table_import_payload: frame %d: zstd body at byte %lld: %s", f, (long long)at,
@@ -559,6 +510,7 @@ TablePtr import_payload_zstd(flockgpu_ctx* handle, const ArrowSchema* schema, co
   std::vector<std::pair<int, int>> ext_col;  // (frame, column) of each pair of ext_req words
   int64_t lit_total = 0, seq_total = 0, src_total = 0, out_total = 0;
   const int64_t n_fields = schema->n_children;
+  const std::vector<size_t> first_buf = field_buffers(schema);
   for (int f = 0; f < n_frames; ++f) {
     FG_CHECK(header_lens[f] >= 0 && (header_lens[f] == 0 || headers[f]), FLOCKGPU_ERR_INVALID, "table_import_payload: frame %d has no header", f);
     FG_CHECK(body_lens[f] >= 0 && (body_lens[f] == 0 || bodies[f]), FLOCKGPU_ERR_INVALID, "table_import_payload: frame %d has no body", f);
@@ -577,16 +529,13 @@ TablePtr import_payload_zstd(flockgpu_ctx* handle, const ArrowSchema* schema, co
     Bd.out = out_total;
     Bd.len = L.body_length;
     Bd.ext_first = int32_t(ext_req.size());
-    size_t next = 0;
-    for (int64_t c = 0; c < n_fields; ++c) {
-      const bool utf8 = dtype_from_format(schema->children[c]->format) == FLOCKGPU_UTF8;
-      if (utf8 && L.length > 0) {
-        ext_req.push_back(Bd.out + L.buffers[next + 1].first);
-        ext_req.push_back(Bd.out + L.buffers[next + 1].first + L.length * 4);
+    for (int64_t c = 0; c < n_fields; ++c)
+      if (dtype_from_format(schema->children[c]->format) == FLOCKGPU_UTF8 && L.length > 0) {
+        const int64_t offs = Bd.out + L.buffers[first_buf[size_t(c)] + 1].first;
+        ext_req.push_back(offs);
+        ext_req.push_back(offs + L.length * 4);
         ext_col.emplace_back(f, int(c));
       }
-      next += utf8 ? 3 : 2;
-    }
     Bd.ext_n = int32_t(ext_req.size()) - Bd.ext_first;
     src_total += body_lens[f];
     out_total += align16(L.body_length);
@@ -673,9 +622,7 @@ TablePtr import_payload_zstd(flockgpu_ctx* handle, const ArrowSchema* schema, co
   std::vector<std::vector<std::pair<int32_t, int32_t>>> extent(size_t(n_frames), std::vector<std::pair<int32_t, int32_t>>(size_t(n_fields), {0, 0}));
   for (size_t k = 0; k < ext_col.size(); ++k) {
     const int f = ext_col[k].first, c = ext_col[k].second;
-    size_t next = 0;
-    for (int i = 0; i < c; ++i) next += dtype_from_format(schema->children[i]->format) == FLOCKGPU_UTF8 ? 3 : 2;
-    check_utf8_extent(f, schema->children[c]->name, ext[2 * k], ext[2 * k + 1], layouts[size_t(f)].buffers[next + 2].second);
+    check_utf8_extent(f, schema->children[c]->name, ext[2 * k], ext[2 * k + 1], layouts[size_t(f)].buffers[first_buf[size_t(c)] + 2].second);
     extent[size_t(f)][size_t(c)] = {ext[2 * k], ext[2 * k + 1]};
   }
 
@@ -685,17 +632,7 @@ TablePtr import_payload_zstd(flockgpu_ctx* handle, const ArrowSchema* schema, co
   t->num_rows = total;
   t->metadata = copy_metadata(schema->metadata);
   std::vector<Seg> segs;
-  // n elements of `unit` destination bytes, cut into pieces of `chunk` elements (a multiple of 8: bitmaps split on bytes)
-  auto add = [&](const uint8_t* s, uint8_t* d, int64_t n, int kind, int32_t arg, int64_t unit, int64_t chunk) {
-    if (kind == 4) {
-      segs.push_back({nullptr, d, 0, kind, arg});
-      return;
-    }
-    for (int64_t k = 0; k < n; k += chunk)
-      segs.push_back({s ? s + (kind == 2 ? k / 8 : k * unit) : nullptr, d + k * unit, std::min(chunk, n - k), kind, arg});
-  };
   const uint8_t* dec = d_dec->as<uint8_t>();
-  constexpr int64_t kChunk = 64 << 10;
   for (int p : proj) {
     const ArrowSchema* cs = schema->children[p];
     const int dt = dtype_from_format(cs->format);
@@ -705,8 +642,7 @@ TablePtr import_payload_zstd(flockgpu_ctx* handle, const ArrowSchema* schema, co
     col.format = cs->format;
     col.nullable = (cs->flags & ARROW_FLAG_NULLABLE) != 0;
     col.length = total;
-    size_t first_buf = 0;
-    for (int i = 0; i < p; ++i) first_buf += dtype_from_format(schema->children[i]->format) == FLOCKGPU_UTF8 ? 3 : 2;
+    const size_t fb = first_buf[size_t(p)];
     bool has_null = false;
     for (const FrameLayout& L : layouts) has_null = has_null || L.nodes[size_t(p)].second > 0;
     if (has_null) col.validity = alloc(ctx, size_t(total));
@@ -727,38 +663,25 @@ TablePtr import_payload_zstd(flockgpu_ctx* handle, const ArrowSchema* schema, co
       const uint8_t* body = dec + zb[size_t(f)].out;
       const int64_t len = L.length;
       if (len == 0) continue;
-      const auto& vbuf = L.buffers[first_buf];
       if (has_null) {
-        if (L.nodes[size_t(p)].second > 0) add(body + vbuf.first, col.validity->as<uint8_t>() + row, len, 2, 0, 1, kChunk);
-        else add(nullptr, col.validity->as<uint8_t>() + row, len, 3, 1, 1, kChunk);
+        if (L.nodes[size_t(p)].second > 0) add_segs(segs, Seg::kBitsToBytes, body + L.buffers[fb].first, col.validity->as<uint8_t>() + row, len);
+        else add_segs(segs, Seg::kFill, nullptr, col.validity->as<uint8_t>() + row, len, 1);
       }
       if (dt == FLOCKGPU_UTF8) {
-        const auto& ob = L.buffers[first_buf + 1];
-        const auto& vb = L.buffers[first_buf + 2];
         const auto ex = extent[size_t(f)][size_t(p)];
-        add(body + ob.first, reinterpret_cast<uint8_t*>(col.offsets->as<int32_t>() + row), len, 1, int32_t(byte - ex.first), 4, kChunk / 4);
-        if (ex.second > ex.first) add(body + vb.first + ex.first, static_cast<uint8_t*>(col.data->ptr) + byte, ex.second - ex.first, 0, 0, 1, kChunk);
+        add_segs(segs, Seg::kOffsets, body + L.buffers[fb + 1].first, reinterpret_cast<uint8_t*>(col.offsets->as<int32_t>() + row), len, int32_t(byte - ex.first));
+        add_segs(segs, Seg::kCopy, body + L.buffers[fb + 2].first + ex.first, static_cast<uint8_t*>(col.data->ptr) + byte, ex.second - ex.first);
         byte += ex.second - ex.first;
       } else {
         const int w = dtype_width(dt);
-        add(body + L.buffers[first_buf + 1].first, static_cast<uint8_t*>(col.data->ptr) + row * w, len * w, 0, 0, 1, kChunk);
+        add_segs(segs, Seg::kCopy, body + L.buffers[fb + 1].first, static_cast<uint8_t*>(col.data->ptr) + row * w, len * w);
       }
       row += len;
     }
-    if (dt == FLOCKGPU_UTF8) add(nullptr, reinterpret_cast<uint8_t*>(col.offsets->as<int32_t>() + total), 0, 4, int32_t(byte), 4, 1);
+    if (dt == FLOCKGPU_UTF8) add_segs(segs, Seg::kSetI32, nullptr, reinterpret_cast<uint8_t*>(col.offsets->as<int32_t>() + total), 1, int32_t(byte));
     t->cols.push_back(std::move(col));
   }
-  BufferPtr d_segs = alloc(ctx, segs.size() * sizeof(Seg));
-  if (!segs.empty()) FG_CUDA(cudaMemcpyAsync(d_segs->ptr, segs.data(), segs.size() * sizeof(Seg), cudaMemcpyHostToDevice, ctx->stream));
-  {
-    LaunchTimer lt(ctx, "payload_assemble_kernel");
-    const int grid = int(std::min<size_t>(std::max<size_t>(segs.size(), 1), size_t(ctx->sm_count) * 16));
-    payload_assemble_kernel<<<grid, 256, 0, ctx->stream>>>(d_segs->as<Seg>(), int(segs.size()));
-  }
-  count_launch(ctx);
-  FG_CUDA(cudaGetLastError());
-  // the segment list is pageable host memory the copy above has already consumed; the scratch buffers are released in
-  // stream order after the launch
+  launch_segments(ctx, segs, "payload_assemble_kernel");  // the scratch buffers are released in stream order after the launch
   return t;
 }
 

@@ -4,15 +4,15 @@
 // `zstd::block::compress(.., 3)` over its header and body on the CPU (flock/src/encoding.rs:72-74).  Here the bodies
 // are laid out, packed and compressed in HBM; only the compressed bytes cross the link.  Frame f holds rows
 // [f * rows_per_frame, min((f + 1) * rows_per_frame, rows)); its uncompressed header and body are exactly what
-// flockgpu_table_export_ipc returns for that row range.
+// flockgpu_table_export_ipc returns for that row range, because both come from pack_frames (host/ipc.cc):
 //
 //   device  payload_layout_kernel  the Utf8 extents and null counts of every (frame, column): one small read-back.
-//   host    body layouts and flatbuffer headers (build_record_batch_message); headers compressed with the shared
-//           encoder functions on the host (zstd_enc.h), as the import decodes them on the host.
-//   device  payload_pack_kernel    one launch over a segment list writes every frame's IPC body: fixed-width values,
-//                                  validity bytes packed into bitmaps, Utf8 offsets rebased to the frame, value bytes
-//                                  (the padding is the zeroed buffer).
-//           zstd_compress_kernel   one CTA per 128 KiB block of every body, every block independent (zstd_enc.h).
+//   host    body layouts and flatbuffer headers.
+//   device  ipc_segment_kernel     one launch over a segment list writes every frame's IPC body in HBM (profiled as
+//                                  payload_pack_kernel).
+//   --- this file ---
+//   host    headers compressed with the shared encoder functions (zstd_enc.h), as the import decodes them on the host.
+//   device  zstd_compress_kernel   one CTA per 128 KiB block of every body, every block independent (zstd_enc.h).
 //           zstd_place_kernel      a scan over the compressed block sizes: each block's place behind its frame header.
 //           zstd_gather_kernel     the blocks' pieces into one contiguous buffer.
 //   copy    one device-to-host copy of the compressed bytes into page-locked memory.
@@ -73,71 +73,6 @@ void zstd_compress_host(const uint8_t* src, int64_t n, std::vector<uint8_t>* out
 }
 
 namespace {
-
-// ---- payload_layout_kernel: one CTA per (frame, column) item -----------------------------------------------------------
-struct LayoutItem {
-  const int32_t* offs;   // Utf8: the column's offsets (else null)
-  const uint8_t* valid;  // a column with a validity buffer (else null)
-  int64_t row, rows;
-};
-
-__global__ void __launch_bounds__(256) payload_layout_kernel(const LayoutItem* __restrict__ items, int n, int64_t* __restrict__ out) {
-  __shared__ unsigned long long nulls;
-  for (int i = blockIdx.x; i < n; i += gridDim.x) {
-    const LayoutItem it = items[i];
-    if (threadIdx.x == 0) nulls = 0;
-    __syncthreads();
-    if (it.valid) {
-      unsigned long long c = 0;
-      for (int64_t r = threadIdx.x; r < it.rows; r += blockDim.x) c += it.valid[it.row + r] == 0;
-      for (int d = 16; d; d >>= 1) c += __shfl_xor_sync(0xFFFFFFFFu, c, d);
-      if ((threadIdx.x & 31) == 0 && c) atomicAdd(&nulls, c);
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      out[3 * i] = it.offs ? it.offs[it.row] : 0;
-      out[3 * i + 1] = it.offs ? it.offs[it.row + it.rows] : 0;
-      out[3 * i + 2] = int64_t(nulls);
-    }
-    __syncthreads();
-  }
-}
-
-// ---- payload_pack_kernel: one CTA per segment -----------------------------------------------------------------------------
-// kind 0: copy n bytes; 1: n int32 offsets, each - arg; 2: n validity bytes -> ceil(n / 8) bitmap bytes.
-struct PackSeg {
-  const uint8_t* src;
-  uint8_t* dst;
-  int64_t n;
-  int32_t kind, arg;
-};
-
-__global__ void __launch_bounds__(256) payload_pack_kernel(const PackSeg* __restrict__ segs, int n_segs) {
-  for (int s = blockIdx.x; s < n_segs; s += gridDim.x) {
-    const PackSeg g = segs[s];
-    const int64_t n = g.n;
-    if (g.kind == 0) {
-      const uintptr_t a = reinterpret_cast<uintptr_t>(g.src) | reinterpret_cast<uintptr_t>(g.dst) | uintptr_t(n);
-      if ((a & 15) == 0) {
-        for (int64_t k = threadIdx.x; k < n / 16; k += blockDim.x) reinterpret_cast<uint4*>(g.dst)[k] = reinterpret_cast<const uint4*>(g.src)[k];
-      } else if ((a & 7) == 0) {
-        for (int64_t k = threadIdx.x; k < n / 8; k += blockDim.x) reinterpret_cast<uint64_t*>(g.dst)[k] = reinterpret_cast<const uint64_t*>(g.src)[k];
-      } else {
-        for (int64_t k = threadIdx.x; k < n; k += blockDim.x) g.dst[k] = g.src[k];
-      }
-    } else if (g.kind == 1) {
-      const int32_t* src = reinterpret_cast<const int32_t*>(g.src);
-      int32_t* dst = reinterpret_cast<int32_t*>(g.dst);
-      for (int64_t r = threadIdx.x; r < n; r += blockDim.x) dst[r] = src[r] - g.arg;
-    } else {
-      for (int64_t k = threadIdx.x; k < (n + 7) / 8; k += blockDim.x) {
-        uint32_t v = 0;
-        for (int j = 0; j < 8 && 8 * k + j < n; ++j) v |= uint32_t(g.src[8 * k + j] != 0) << j;
-        g.dst[k] = uint8_t(v);
-      }
-    }
-  }
-}
 
 // ---- zstd_compress_kernel: one CTA per block ------------------------------------------------------------------------------
 struct EncBlock {
@@ -246,7 +181,6 @@ __global__ void __launch_bounds__(256) zstd_gather_kernel(const zs::BlockOut* __
 }
 
 int64_t align16(int64_t x) { return (x + 15) & ~int64_t(15); }
-int64_t pad8(int64_t x) { return (x + 7) & ~int64_t(7); }
 
 }  // namespace
 
@@ -277,107 +211,26 @@ void export_payload(const CtxPtr& ctx, const Table& t, int32_t encoding, int64_t
   const int n_frames = int(rows == 0 ? 0 : (rows + rows_per_frame - 1) / rows_per_frame);
   FG_CHECK(rows / rows_per_frame < (int64_t(1) << 30), FLOCKGPU_ERR_INVALID, "table_export_payload: %lld frames", (long long)(rows / rows_per_frame));
   if (n_frames == 0) return;
-  const size_t n_cols = t.cols.size();
-  auto frame_rows = [&](int f) { return std::min(rows_per_frame, rows - int64_t(f) * rows_per_frame); };
-
-  // ---- layout: Utf8 extents and null counts of every (frame, column), one read-back ----
-  std::vector<LayoutItem> items;
-  std::vector<int32_t> item_of(size_t(n_frames) * n_cols, -1);
-  for (int f = 0; f < n_frames; ++f)
-    for (size_t i = 0; i < n_cols; ++i) {
-      const Column& c = t.cols[i];
-      const bool utf8 = c.dtype == FLOCKGPU_UTF8;
-      const bool some_null = !c.all_null && c.validity;
-      if (!utf8 && !some_null) continue;
-      item_of[size_t(f) * n_cols + i] = int32_t(items.size());
-      items.push_back({utf8 ? c.offs() : nullptr, some_null ? c.valid() : nullptr, int64_t(f) * rows_per_frame, frame_rows(f)});
-    }
-  std::vector<int64_t> lay(items.size() * 3);
-  if (!items.empty()) {
-    BufferPtr d_items = alloc(ctx, items.size() * sizeof(LayoutItem));
-    BufferPtr d_lay = alloc(ctx, lay.size() * 8);
-    FG_CUDA(cudaMemcpyAsync(d_items->ptr, items.data(), items.size() * sizeof(LayoutItem), cudaMemcpyHostToDevice, ctx->stream));
-    {
-      LaunchTimer lt(ctx, "payload_layout_kernel");
-      const int grid = int(std::min<size_t>(items.size(), size_t(ctx->sm_count) * 16));
-      payload_layout_kernel<<<grid, 256, 0, ctx->stream>>>(d_items->as<LayoutItem>(), int(items.size()), d_lay->as<int64_t>());
-    }
-    count_launch(ctx);
-    FG_CUDA(cudaGetLastError());
-    FG_CUDA(cudaMemcpyAsync(lay.data(), d_lay->ptr, lay.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    FG_CUDA(cudaStreamSynchronize(ctx->stream));
-  }
-
-  // ---- host: body layouts (as export_ipc_frame lays them out), headers, pack segments ----
-  const size_t nf = static_cast<size_t>(n_frames);
-  std::vector<int64_t> body_at(nf), body_len(nf);
-  std::vector<std::vector<uint8_t>> headers(nf);
-  std::vector<PackSeg> segs;
-  int64_t packed = 0;
-  constexpr int64_t kChunk = 64 << 10;
-  auto add = [&](const uint8_t* s, int64_t dst_off, int64_t n, int kind, int32_t arg) {
-    // kind 0: n bytes; 1: n int32 words; 2: n rows (a multiple of 8 per piece, so bitmaps split on bytes)
-    const int64_t unit = kind == 1 ? 4 : 1;
-    for (int64_t k = 0; k < n; k += kChunk)
-      segs.push_back({s + k * unit, reinterpret_cast<uint8_t*>(dst_off + (kind == 2 ? k / 8 : k * unit)), std::min(kChunk, n - k), kind, arg});
-  };
-  for (int f = 0; f < n_frames; ++f) {
-    const int64_t rb = int64_t(f) * rows_per_frame, rc = frame_rows(f);
-    std::vector<std::pair<int64_t, int64_t>> nodes, buffers;
-    int64_t len = 0;
-    body_at[size_t(f)] = packed;
-    for (size_t i = 0; i < n_cols; ++i) {
-      const Column& c = t.cols[i];
-      const int it = item_of[size_t(f) * n_cols + i];
-      const bool all_null = c.all_null;
-      const bool some_null = !all_null && c.validity;
-      nodes.emplace_back(rc, all_null ? rc : some_null ? lay[size_t(it) * 3 + 2] : 0);
-      const int64_t vbytes = (all_null || some_null) ? (rc + 7) / 8 : 0;
-      buffers.emplace_back(len, vbytes);
-      if (some_null) add(c.valid() + rb, packed + len, rc, 2, 0);
-      len += pad8(vbytes);
-      if (c.dtype == FLOCKGPU_UTF8) {
-        const int32_t first = int32_t(lay[size_t(it) * 3]), last = int32_t(lay[size_t(it) * 3 + 1]);
-        buffers.emplace_back(len, (rc + 1) * 4);
-        add(reinterpret_cast<const uint8_t*>(c.offs() + rb), packed + len, rc + 1, 1, first);
-        len += pad8((rc + 1) * 4);
-        buffers.emplace_back(len, int64_t(last - first));
-        if (last > first) add(static_cast<const uint8_t*>(c.values()) + first, packed + len, last - first, 0, 0);
-        len += pad8(int64_t(last - first));
-      } else {
-        buffers.emplace_back(len, rc * c.width());
-        if (!all_null) add(static_cast<const uint8_t*>(c.values()) + rb * c.width(), packed + len, rc * c.width(), 0, 0);
-        len += pad8(rc * c.width());
-      }
-    }
-    FG_CHECK(encoding != FLOCKGPU_ENCODING_ZSTD || len <= kMaxZstdBody, FLOCKGPU_ERR_INVALID,
+  std::vector<std::pair<int64_t, int64_t>> ranges;
+  for (int f = 0; f < n_frames; ++f) ranges.emplace_back(int64_t(f) * rows_per_frame, std::min(rows_per_frame, rows - int64_t(f) * rows_per_frame));
+  const PackedFrames B = pack_frames(ctx, t, ranges);
+  const std::vector<int64_t>& body_at = B.body_at;
+  const std::vector<int64_t>& body_len = B.body_len;
+  const uint8_t* bodies = B.bodies->as<uint8_t>();
+  const int64_t packed = body_at.back() + align16(body_len.back());
+  for (int f = 0; f < n_frames && encoding == FLOCKGPU_ENCODING_ZSTD; ++f) {
+    const int64_t rb = ranges[size_t(f)].first, rc = ranges[size_t(f)].second, len = body_len[size_t(f)];
+    FG_CHECK(len <= kMaxZstdBody, FLOCKGPU_ERR_INVALID,
              "table_export_payload: frame %d (rows %lld..%lld) has a %lld-byte body; a zstd frame's body must stay within %lld bytes (pick fewer rows per frame)", f,
              (long long)rb, (long long)(rb + rc), (long long)len, (long long)kMaxZstdBody);
-    body_len[size_t(f)] = len;
-    headers[size_t(f)] = build_record_batch_message(rc, nodes, buffers, len);
-    packed += align16(len);
   }
-  BufferPtr d_bodies = alloc(ctx, size_t(std::max<int64_t>(packed, 16)));
-  uint8_t* bodies = d_bodies->as<uint8_t>();
-  for (PackSeg& s : segs) s.dst = bodies + reinterpret_cast<int64_t>(s.dst);
-  FG_CUDA(cudaMemsetAsync(bodies, 0, size_t(packed), ctx->stream));
-  BufferPtr d_segs = alloc(ctx, segs.size() * sizeof(PackSeg));
-  ctx->h2d_bytes.fetch_add(int64_t(segs.size() * sizeof(PackSeg)), std::memory_order_relaxed);
-  if (!segs.empty()) FG_CUDA(cudaMemcpyAsync(d_segs->ptr, segs.data(), segs.size() * sizeof(PackSeg), cudaMemcpyHostToDevice, ctx->stream));
-  {
-    LaunchTimer lt(ctx, "payload_pack_kernel");
-    const int grid = int(std::min<size_t>(std::max<size_t>(segs.size(), 1), size_t(ctx->sm_count) * 16));
-    payload_pack_kernel<<<grid, 256, 0, ctx->stream>>>(d_segs->as<PackSeg>(), int(segs.size()));
-  }
-  count_launch(ctx);
-  FG_CUDA(cudaGetLastError());
 
   // headers: the flatbuffers themselves, or compressed on the host
   P->frames.resize(size_t(n_frames));
   {
     HostEncoder enc;
     for (int f = 0; f < n_frames; ++f) {
-      const std::vector<uint8_t>& h = headers[size_t(f)];
+      const std::vector<uint8_t>& h = B.headers[size_t(f)];
       P->frames[size_t(f)].header_at = int64_t(P->headers.size());
       if (encoding == FLOCKGPU_ENCODING_ZSTD) enc.compress(h.data(), int64_t(h.size()), &P->headers);
       else P->headers.insert(P->headers.end(), h.begin(), h.end());

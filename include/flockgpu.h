@@ -151,7 +151,8 @@ int flockgpu_table_export(flockgpu_ctx* ctx, const flockgpu_table* table, int64_
 /* Host -> HBM from `n_frames` DataFrame { header, body } pairs (Encoding::None): header = the flatbuffer Message of a
  * RecordBatch (FlightData.data_header), body = its buffers (FlightData.data_body).  Nothing is decoded: the body
  * buffers are the column buffers, only their extents are read from the header.  `schema` / `projection` as in
- * flockgpu_table_import; frames with nulls, dictionaries or compressed bodies are rejected (FLOCKGPU_ERR_UNSUPPORTED). */
+ * flockgpu_table_import; frames with dictionaries or compressed bodies are rejected (FLOCKGPU_ERR_UNSUPPORTED).
+ * Columns with nulls import: their validity bitmaps become the table's validity. */
 int flockgpu_table_import_ipc(flockgpu_ctx* ctx, const struct ArrowSchema* schema, const uint8_t* const* headers, const int64_t* header_lens,
                               const uint8_t* const* bodies, const int64_t* body_lens, int32_t n_frames, const int32_t* projection,
                               int32_t n_projection, flockgpu_table** out);

@@ -1,7 +1,8 @@
 """flockgpu_table_export_payload on the GPU: a table in HBM becomes a payload's DataFrames, each body packed and
 zstd-compressed on the device.  Every frame decompresses (pyarrow / libzstd) to what to_ipc gives for its row range,
-every zstd body is byte for byte the host self test's output for that uncompressed body, the import takes the frames
-back to the same table, and only compressed bytes cross the link."""
+pyarrow's IPC reader reads every uncompressed frame as the table's rows, every zstd body is byte for byte the host
+self test's output for that uncompressed body, the import takes the frames back to the same table, and only
+compressed bytes cross the link."""
 import numpy as np
 import pyarrow as pa
 import pytest
@@ -99,10 +100,15 @@ def _round_trip(ctx, t: fb.Table, rows_per_frame: int) -> None:
     zs = t.to_payload("zstd", rows_per_frame)
     assert len(zs) == -(-t.num_rows // rows_per_frame)
     plain = t.to_payload("none", rows_per_frame)
+    table = t.to_arrow()
     for f, ((zh, zb), (h, b)) in enumerate(zip(zs, plain)):
+        n = min(rows_per_frame, t.num_rows - f * rows_per_frame)
         assert _unz(zh) == h and _unz(zb) == b and zb == fb.selftest_zstd_compress(b), (rows_per_frame, f)
-        assert (h, b) == t.to_ipc(f * rows_per_frame, min(rows_per_frame, t.num_rows - f * rows_per_frame))
-    schema = t.to_arrow().schema
+        assert (h, b) == t.to_ipc(f * rows_per_frame, n)
+        got, want = _read(h, b, table.schema), table.slice(f * rows_per_frame, n)
+        assert pa.Table.from_batches([got]).equals(want), (rows_per_frame, f)
+        assert [c.null_count for c in got.columns] == [c.null_count for c in want.columns], (rows_per_frame, f)
+    schema = table.schema
     back = ctx.import_payload(schema, zs)
     _same(back, t)
     _same(ctx.import_payload(schema, plain, encoding="none"), t)
@@ -111,6 +117,13 @@ def _round_trip(ctx, t: fb.Table, rows_per_frame: int) -> None:
 def test_round_trip_every_column_type_with_nulls(gpu_ctx):
     rng = np.random.default_rng(5)
     t = gpu_ctx.import_batches([_all_types_batch(10_007, rng)])
+    # validity crosses the link as bitmaps, not a byte per row: the body plus the layout read-back (24 B per column that
+    # is Utf8 or has NULLs)
+    laid_out = sum(1 for c in t.to_arrow().columns if c.null_count or pa.types.is_string(c.type))
+    d2h = gpu_ctx.bytes_moved()[1]
+    _, body = t.to_ipc()
+    d2h = gpu_ctx.bytes_moved()[1] - d2h
+    assert d2h <= len(body) + 24 * laid_out, (d2h, len(body))
     for rows_per_frame in (1, 7, 4096, 65536, 20_000):
         if rows_per_frame == 1:
             _round_trip(gpu_ctx, gpu_ctx.import_batches([_all_types_batch(40, rng)]), 1)
