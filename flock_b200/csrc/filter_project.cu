@@ -70,6 +70,54 @@ struct PredGenericT {
 };
 
 
+// other JOIN (group key, MIN / MAX) ON (k, v) against a direct-address group table (NEXMark q9: bids back to each
+// auction's top price): a row survives when k is inside the table's range, its slot is present and the slot's value
+// equals v; a NULL k or v matches nothing.  The table (q9: 600 K auctions, a byte and a word each) stays in L2 while
+// the two columns stream once.  Every thread issues all its rows' loads before it tests any of them.
+struct PredGroupMatch {
+  static constexpr int E = 1;
+  static constexpr int I = 16;
+  static constexpr int MIN_CTAS = 2;
+  static constexpr bool ROUNDS = false;
+  struct Staged {};
+  const uint32_t* key;
+  const void* val;
+  const uint8_t* key_valid;
+  const uint8_t* val_valid;
+  int32_t val_width;  // 4 or 8
+  int32_t pad;
+  GroupMatchTable t;
+  __device__ __forceinline__ void load(Staged&, int64_t, int64_t, int) const {}
+  __device__ __forceinline__ unsigned long long test(const Staged&, const ColRef*, int64_t tile_base, int64_t n_rows, int tid, int*) const {
+    unsigned long long slot[I], v[I];
+    unsigned ok = 0;
+#pragma unroll
+    for (int k = 0; k < I; ++k) {
+      const int64_t r = tile_base + int64_t(k) * FP_THREADS + tid;
+      slot[k] = ~0ull;
+      v[k] = 0;
+      if (r < n_rows) {
+        slot[k] = (unsigned long long)key[r] - t.base;  // keys below the base wrap to huge slots
+        v[k] = val_width == 4 ? (unsigned long long)static_cast<const uint32_t*>(val)[r] : static_cast<const unsigned long long*>(val)[r];
+        const bool null_row = (key_valid && !key_valid[r]) || (val_valid && !val_valid[r]);
+        if (!null_row && slot[k] < t.n_slots) ok |= 1u << k;
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < I; ++k)
+      if (((ok >> k) & 1u) && !t.present[slot[k]]) ok &= ~(1u << k);
+    unsigned long long bits = 0;
+#pragma unroll
+    for (int k = 0; k < I; ++k) {
+      if (!((ok >> k) & 1u)) continue;
+      const unsigned long long a = t.acc[slot[k]];
+      const bool eq = val_width == 4 ? uint32_t(a) == uint32_t(v[k]) : a == v[k];
+      if (eq && (!t.valid || t.valid[slot[k]] != 0ull)) bits |= 1ull << k;
+    }
+    return bits;
+  }
+};
+
 // One tile = 8 Ki rows: every thread copies eight 16-byte pieces of the column per tile into shared memory with
 // cp.async, and the kernel keeps the next tile's copies in flight while it ranks, publishes and writes the current
 // one (cooperative rounds, compact.cuh).  Staging in shared memory instead of registers keeps the loads in flight
@@ -448,7 +496,7 @@ static void fill_colrefs(const Table& t, ColRef* refs) {
 // of the instantiation launched: functors with ROUNDS walk any number of cooperative rounds; the others run one
 // wave when the tiles fit it and fall back to decoupled look-back beyond it.
 template <class PredFn, bool COMPUTED>
-static void launch_filter(const CtxPtr& ctx, const PredFn& pred, FilterArgs args) {
+static void launch_filter(const CtxPtr& ctx, const PredFn& pred, FilterArgs args, const char* profile_name = "filter_compact_kernel") {
   constexpr int64_t TILE = int64_t(FP_THREADS) * PredFn::I;
   const int64_t num_tiles = (args.n_rows + TILE - 1) / TILE;
   auto* kernel = &filter_compact_kernel<PredFn, COMPUTED>;
@@ -464,7 +512,7 @@ static void launch_filter(const CtxPtr& ctx, const PredFn& pred, FilterArgs args
     args.trace = trace_buf->as<unsigned long long>();
   }
   {
-    LaunchTimer lt(ctx, "filter_compact_kernel");
+    LaunchTimer lt(ctx, profile_name);
     launch_compact(ctx, kernel, args.sc, pred, args);
   }
   FG_CUDA(cudaGetLastError());
@@ -789,6 +837,65 @@ TablePtr filter_project(const CtxPtr& ctx, const TablePtr& in_ptr, const Expr* p
     for (size_t u = 0; u < utf8_outs.size(); ++u) {
       g[u].name = out->cols[utf8_outs[u]].name;
       out->cols[utf8_outs[u]] = std::move(g[u]);
+    }
+  }
+  return out;
+}
+
+TablePtr select_group_match_rows(const CtxPtr& ctx, const Table& in, int key_col, int val_col, const GroupMatchTable& t) {
+  in.dense();
+  if (in.num_rows == 0) return empty_like(ctx, in);
+  FilterArgs fa{};
+  fa.n_rows = in.num_rows;
+  fa.out_count = ctx->d_scalars + 0;
+  fa.err_flag = reinterpret_cast<int*>(ctx->d_scalars + 8);
+  fill_colrefs(in, fa.cols);
+  auto out = std::make_shared<Table>();
+  out->ctx = ctx;
+  out->metadata = in.metadata;
+  std::vector<int> sel_outs;  // Utf8 columns and columns with validity bytes leave through the selection vector
+  for (size_t i = 0; i < in.cols.size(); ++i) {
+    const Column& s = in.cols[i];
+    Column c;
+    c.name = s.name;
+    c.dtype = s.dtype;
+    c.format = s.format;
+    c.nullable = s.nullable;
+    if (s.dtype == FLOCKGPU_UTF8 || s.validity) {
+      sel_outs.push_back(int(i));
+    } else {
+      FG_CHECK(fa.n_out < MAX_OUT_COLS, FLOCKGPU_ERR_UNSUPPORTED, "join: more than %d fixed-width output columns", MAX_OUT_COLS);
+      c.data = alloc(ctx, size_t(in.num_rows) * s.width());
+      OutCol& oc = fa.outs[fa.n_out++];
+      oc.kind = OUT_PASS;
+      oc.src_col = int(i);
+      oc.out_dtype = s.dtype;
+      oc.width = s.width();
+      oc.dst = c.data->ptr;
+    }
+    out->cols.push_back(std::move(c));
+  }
+  BufferPtr sel;
+  if (!sel_outs.empty()) {
+    sel = alloc(ctx, size_t(in.num_rows) * 4);
+    fa.sel_out = sel->as<uint32_t>();
+  }
+  const Column& k = in.cols[key_col];
+  const Column& v = in.cols[val_col];
+  PredGroupMatch pred{static_cast<const uint32_t*>(k.values()), v.values(), k.valid(), v.valid(), v.width(), 0, t};
+  launch_filter<PredGroupMatch, false>(ctx, pred, fa, "group_match_kernel");  // its own name in the launch profile
+  unsigned long long n_sel = 0;
+  read_scalars(ctx, 0, 1, &n_sel);
+  FG_CHECK(int64_t(n_sel) <= in.num_rows, FLOCKGPU_ERR_CUDA, "join: corrupt survivor count %llu", n_sel);
+  out->num_rows = int64_t(n_sel);
+  for (Column& c : out->cols) c.length = out->num_rows;
+  if (!sel_outs.empty()) {
+    std::vector<const Column*> src;
+    for (int i : sel_outs) src.push_back(&in.cols[i]);
+    std::vector<Column> g = gather_columns(ctx, src, fa.sel_out, out->num_rows);
+    for (size_t u = 0; u < sel_outs.size(); ++u) {
+      g[u].name = out->cols[sel_outs[u]].name;
+      out->cols[sel_outs[u]] = std::move(g[u]);
     }
   }
   return out;

@@ -2488,6 +2488,132 @@ static TablePtr emit_groups(const CtxPtr& ctx, const Table& in, const std::vecto
   return out;
 }
 
+// ---- a SINGLE aggregate by one 4-byte key with MIN / MAX whose level-2 table is direct-address stays in that table
+// (NEXMark q9: each auction's MAX(price), which the outer join on (auction, price) reads back per bid).  The join asks
+// select_group_match for one selection over its other side; every other consumer materialises exactly the rows the
+// emit path writes.
+namespace {
+
+struct GroupsCore {
+  CtxPtr ctx;
+  TablePtr input;
+  std::vector<int> group_cols;
+  std::vector<AggSpec> aggs;
+  AggPlan plan;
+  GroupTable table;
+  TablePtr full;  // the emitted rows, produced at most once
+  TablePtr materialise_full() {
+    if (!full) full = emit_groups(ctx, *input, group_cols, plan, table);
+    return full;
+  }
+};
+
+struct DeferredGroups : DeferredTable {
+  std::shared_ptr<GroupsCore> core;
+  std::vector<int> kinds;  // per visible column: its column of the emitted relation (0 = the key, 1 + j = output j)
+  void materialise(const Table& self) override {
+    TablePtr f = core->materialise_full();
+    self.num_rows = f->num_rows;
+    for (size_t i = 0; i < kinds.size(); ++i) {
+      Column c = f->cols[kinds[i]];
+      c.name = self.cols[i].name;
+      self.cols[i] = std::move(c);
+    }
+  }
+  TablePtr project(const Table& self, const std::vector<int>& src_cols, const std::vector<std::string>& names) override;
+  TablePtr select_group_match(const Table& self, const int (&self_keys)[2], const TablePtr& other, const int (&other_keys)[2],
+                              bool self_is_left) override;
+};
+
+TablePtr groups_table(const std::shared_ptr<GroupsCore>& core, const std::vector<int>& kinds, const std::vector<std::string>& names,
+                      const std::string& metadata) {
+  auto t = std::make_shared<Table>();
+  t->ctx = core->ctx;
+  t->metadata = metadata;
+  t->num_rows = -1;
+  for (size_t i = 0; i < kinds.size(); ++i) {
+    Column c;
+    if (kinds[i] == 0) {
+      c = key_out_col(*core->input, core->group_cols[0], -1);
+    } else {
+      const OutPlan& o = core->plan.outs[kinds[i] - 1];
+      c.dtype = o.dtype;
+      c.format = o.format;
+      c.nullable = true;
+      c.length = -1;
+    }
+    c.name = names[i];
+    t->cols.push_back(std::move(c));
+  }
+  auto d = std::make_shared<DeferredGroups>();
+  d->core = core;
+  d->kinds = kinds;
+  t->deferred = d;
+  return t;
+}
+
+TablePtr DeferredGroups::project(const Table& self, const std::vector<int>& src_cols, const std::vector<std::string>& names) {
+  std::vector<int> k;
+  for (int c : src_cols) k.push_back(kinds[c]);
+  return groups_table(core, k, names, self.metadata);
+}
+
+TablePtr DeferredGroups::select_group_match(const Table& self, const int (&self_keys)[2], const TablePtr& other_ptr, const int (&other_keys)[2],
+                                            bool self_is_left) {
+  for (int i = 0; i < 2; ++i)
+    if (self_keys[i] < 0 || self_keys[i] >= int(kinds.size())) return nullptr;
+  // which of the two key pairs is (group column, other column) and which (aggregate, other column)
+  const int kp = kinds[self_keys[0]] == 0 ? 0 : 1, vp = 1 - kp;
+  if (kinds[self_keys[kp]] != 0 || kinds[self_keys[vp]] == 0) return nullptr;
+  const int out_col = kinds[self_keys[vp]];
+  const OutPlan& o = core->plan.outs[out_col - 1];
+  const int func = core->aggs[out_col - 1].func;
+  if ((func != FLOCKGPU_AGG_MIN && func != FLOCKGPU_AGG_MAX) || o.kind != EMIT_RAW || o.dtype == FLOCKGPU_FLOAT64) return nullptr;
+  // every column of self must be one of the two: both are the survivors' own values
+  for (int k : kinds)
+    if (k != 0 && k != out_col) return nullptr;
+  const Table& other = *other_ptr;
+  other.dense();
+  const int ok = other_keys[kp], ov = other_keys[vp];
+  if (ok < 0 || ok >= int(other.cols.size()) || ov < 0 || ov >= int(other.cols.size())) return nullptr;
+  const Column& key = core->input->cols[core->group_cols[0]];
+  if (other.cols[ok].dtype != key.dtype || other.cols[ov].dtype != o.dtype || other.cols[ok].all_null || other.cols[ov].all_null) return nullptr;
+  const AggEmitArgs& ea = core->table.ea;
+  GroupMatchTable gt{ea.present, ea.acc + o.a0 * ea.acc_stride, o.valid_acc >= 0 ? ea.acc + o.valid_acc * ea.acc_stride : nullptr, ea.dense_base,
+                     ea.n_slots - 1};
+  TablePtr rows = select_group_match_rows(core->ctx, other, ok, ov, gt);
+  // self's columns are views of the survivors' key and value columns (equal by the join condition, and never NULL)
+  std::vector<Column> mine;
+  for (size_t i = 0; i < kinds.size(); ++i) {
+    Column c = rows->cols[kinds[i] == 0 ? ok : ov];
+    c.name = self.cols[i].name;
+    c.format = self.cols[i].format;
+    c.nullable = self.cols[i].nullable;
+    c.validity = nullptr;
+    mine.push_back(std::move(c));
+  }
+  auto t = std::make_shared<Table>();
+  t->ctx = core->ctx;
+  t->metadata = self_is_left ? self.metadata : other.metadata;
+  t->num_rows = rows->num_rows;
+  if (self_is_left) {
+    t->cols = std::move(mine);
+    for (const Column& c : rows->cols) t->cols.push_back(c);
+  } else {
+    t->cols = rows->cols;
+    for (Column& c : mine) t->cols.push_back(std::move(c));
+  }
+  return t;
+}
+
+bool has_minmax(const std::vector<AggSpec>& aggs) {
+  for (const AggSpec& s : aggs)
+    if (s.func == FLOCKGPU_AGG_MIN || s.func == FLOCKGPU_AGG_MAX) return true;
+  return false;
+}
+
+}  // namespace
+
 // The decision tree of DESIGN.md K5-K7: no group columns -> one row; empty input -> empty output; packed keys -> the
 // direct-address count table, else level-1 partials (large raw inputs) and the level-2 table; other keys -> the
 // row-representative table.
@@ -2529,6 +2655,22 @@ static TablePtr hash_aggregate_impl(const CtxPtr& ctx, const TablePtr& in_ptr, i
       l1 = level1_partials(ctx, in, kp, p, count32);
     }
     t = packed_table(ctx, in, kp, p, l1);
+    if (t.mode == 1 && allow_dense && mode == FLOCKGPU_AGG_SINGLE && kp.n == 1 && kp.width[0] == 4 && has_minmax(aggs) && comm_world(ctx) == 1) {
+      auto core = std::make_shared<GroupsCore>();
+      core->ctx = ctx;
+      core->input = in_ptr;
+      core->group_cols = group_cols;
+      core->aggs = aggs;
+      core->plan = p;
+      core->table = std::move(t);
+      std::vector<int> kinds{0};
+      std::vector<std::string> names{in.cols[group_cols[0]].name};
+      for (size_t j = 0; j < p.outs.size(); ++j) {
+        kinds.push_back(int(j) + 1);
+        names.push_back(p.outs[j].name);
+      }
+      return groups_table(core, kinds, names, in.metadata);
+    }
   } else if (TablePtr distinct = row_table(ctx, in, group_cols, p, &t)) {
     return distinct;
   }

@@ -358,6 +358,15 @@ TablePtr hash_join(const CtxPtr& ctx, const TablePtr& left_ptr, const TablePtr& 
     if (std::shared_ptr<DeferredTable> d = right_ptr->deferred)
       if (TablePtr t = d->select_equal(R, right_keys[0], left_ptr, left_keys[0], false)) return t;
   }
+  // one side is a (key, MIN / MAX) group-by still in its direct-address table and the join is on (key, MIN / MAX)
+  // (NEXMark q9: bids back to each auction's top price): one selection over the other side, no hash table
+  if (left_keys.size() == 2 && right_keys.size() == 2) {
+    const int lk[2] = {left_keys[0], left_keys[1]}, rk[2] = {right_keys[0], right_keys[1]};
+    if (std::shared_ptr<DeferredTable> d = right_ptr->deferred)
+      if (TablePtr t = d->select_group_match(R, rk, left_ptr, lk, false)) return t;
+    if (std::shared_ptr<DeferredTable> d = left_ptr->deferred)
+      if (TablePtr t = d->select_group_match(L, lk, right_ptr, rk, true)) return t;
+  }
   L.dense();
   R.dense();
   FG_CHECK(!left_keys.empty() && left_keys.size() == right_keys.size(), FLOCKGPU_ERR_INVALID, "hash_join: key lists must be non-empty and of equal length");

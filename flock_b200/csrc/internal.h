@@ -333,7 +333,24 @@ struct DeferredTable {
   virtual TablePtr global_max(const Table& self, int col, const std::string& out_name) { return nullptr; }
   // self JOIN one_row ON self.key_col = one_row.one_key, output columns self ++ one_row (or the reverse):
   virtual TablePtr select_equal(const Table& self, int key_col, const TablePtr& one_row, int one_key, bool self_is_left) { return nullptr; }
+  // other JOIN self ON other.keys[0] = self.self_keys[0] AND other.keys[1] = self.self_keys[1], where the pair is
+  // (group column, MIN / MAX column) in either order; output columns other ++ self (or the reverse):
+  virtual TablePtr select_group_match(const Table& self, const int (&self_keys)[2], const TablePtr& other, const int (&other_keys)[2],
+                                      bool self_is_left) { return nullptr; }
 };
+
+// A direct-address (key, MIN / MAX) table as the matching selection reads it: slot = key - base for a 4-byte key,
+// present[slot] != 0 for a group that exists, acc[slot] its MIN / MAX (int64 for a signed column: compared in the
+// value column's width) and, when the aggregated column had NULLs, valid[slot] = its non-NULL count (0: the MAX is NULL).
+struct GroupMatchTable {
+  const unsigned char* present;
+  const unsigned long long* acc;
+  const unsigned long long* valid;
+  unsigned long long base, n_slots;
+};
+// The rows of `other` whose column `key_col` names a group of `t` and whose `val_col` equals that group's value, in
+// row order, with every column of `other` (filter_project.cu: filter_compact_kernel with the group_match predicate).
+TablePtr select_group_match_rows(const CtxPtr& ctx, const Table& other, int key_col, int val_col, const GroupMatchTable& t);
 
 struct Table {
   CtxPtr ctx;

@@ -254,6 +254,40 @@ def persons(n_persons: int, seed: int = 42, first_person: int = 0, columns: list
     return pa.RecordBatch.from_arrays(arrays, schema=pa.schema(fields, metadata=full.metadata))
 
 
+TS_NS_UTC = pa.timestamp("ns", tz="UTC")
+
+
+def bid_ptime_schema() -> pa.Schema:
+    """The bid columns plus the processing time q12 groups by: ``SELECT *, now() AS p_time FROM bid``."""
+    return pa.schema(list(bid_schema()) + [pa.field("p_time", TS_NS_UTC, False)], metadata={"name": "bid"})
+
+
+def bids_ptime(n_bids: int, seed: int = 42, first_bid: int = 0) -> pa.RecordBatch:
+    """``bids(n_bids, seed, first_bid)`` with a ``p_time`` column.  The reference stamps every bid with ``now()`` as its
+    source function reads it; here the stamp is deterministic: it advances by 1 us every 4 bids (monotone in the bid's
+    position, 4 bids per stamp), so each bidder's MIN and MAX are stamps of different bids."""
+    b = bids(n_bids, seed, first_bid)
+    k = np.arange(first_bid, first_bid + n_bids, dtype=np.int64)
+    p_time = pa.array(BASE_TIME * 1_000_000 + (k // 4) * 1_000, TS_NS_UTC)
+    return pa.RecordBatch.from_arrays(list(b.columns) + [p_time], schema=bid_ptime_schema())
+
+
+def side_input_schema() -> pa.Schema:
+    """event.rs:375-385"""
+    return pa.schema([pa.field("key", pa.int32(), False), pa.field("value", pa.int32(), False)], metadata={"name": "side_input"})
+
+
+def side_input(n_auctions: int, seed: int = 42) -> pa.RecordBatch:
+    """q13's side input, SYNTHETIC: the reference downloads a CSV of (key, value) pairs; this table is generated from
+    ``seed`` instead.  Keys are the auction ids a window of ``n_auctions`` auctions produces, ascending, with about one
+    in eight left out so that some bids find no match; values are uniform in [0, 2^20)."""
+    rng = np.random.default_rng([seed, 4])
+    ids = np.arange(FIRST_AUCTION_ID, FIRST_AUCTION_ID + n_auctions, dtype=np.int32)
+    keys = ids[rng.random(ids.size) >= 0.125]
+    values = rng.integers(0, 1 << 20, keys.size).astype(np.int32)
+    return pa.RecordBatch.from_arrays([pa.array(keys), pa.array(values)], schema=side_input_schema())
+
+
 def bids_chunked(n_bids: int, seed: int = 42, columns: list[str] | None = None, first_bid: int = 0, chunk: int = 4_000_000,
                  threads: int = 16, batch_rows: int = BATCH_ROWS) -> list[pa.RecordBatch]:
     """``n_bids`` consecutive bids generated ``chunk`` at a time on a thread pool (numpy releases the interpreter lock

@@ -278,9 +278,81 @@ def q6(n: int = TARGET_PARTITIONS) -> dict:
     return projection_exec([(column("seller", 0), "seller"), (column("AVG(R.price)", 1), "AVG(R.price)")], outer)
 
 
+# ---- NEXMark q0 / q10, q9, q12, q13 ----------------------------------------------------------------------------------
+BID_PTIME, SIDE_INPUT = nexgen.bid_ptime_schema(), nexgen.side_input_schema()
+TS_NS_UTC = {"Timestamp": ["Nanosecond", "UTC"]}
+
+
+def q10(n: int = TARGET_PARTITIONS) -> dict:
+    """benchmarks/src/nexmark/query/q10.sql (q0.sql is the same query):  SELECT auction, bidder, price, b_date_time FROM bid"""
+    scan = repartition_rr(memory_exec(BID, [0, 1, 2, 3]), n)
+    return projection_exec([(column("auction", 0), "auction"), (column("bidder", 1), "bidder"), (column("price", 2), "price"),
+                            (column("b_date_time", 3), "b_date_time")], scan)
+
+
+q0 = q10
+
+
+def q9(n: int = TARGET_PARTITIONS) -> dict:
+    """benchmarks/src/nexmark/query/q9.sql, types q9_plan.fmt:
+       SELECT auction, bidder, price, b_date_time FROM bid JOIN (SELECT a_id AS id, MAX(price) AS final FROM auction
+       JOIN bid ON a_id = auction WHERE b_date_time BETWEEN a_date_time AND expires GROUP BY a_id) AS Q
+       ON auction = id AND price = final.
+    The inner part is q4's join and BETWEEN filter grouped by a_id alone; the outer join is Partitioned on the key pair,
+    both sides Hash-repartitioned on it.  The BETWEEN filter applies to the subquery only: the outer join keeps every
+    bid at its auction's top price, in the auction's lifetime or not."""
+    a_scan = repartition_rr(memory_exec(AUCTION, [0, 5, 6]), n)        # a_id, a_date_time, expires
+    b_scan = repartition_rr(memory_exec(BID, [0, 1, 2, 3]), n)         # auction, bidder, price, b_date_time
+    lsh = coalesce_batches_exec(repartition_hash(a_scan, [column("a_id", 0)], n))
+    rsh = coalesce_batches_exec(repartition_hash(b_scan, [column("auction", 0)], n))
+    join = coalesce_batches_exec(hash_join_exec(lsh, rsh, [(column("a_id", 0), column("auction", 0))]))
+    # a_id 0, a_date_time 1, expires 2, auction 3, bidder 4, price 5, b_date_time 6
+    between = binary(binary(column("b_date_time", 6), "GtEq", column("a_date_time", 1)), "And",
+                     binary(column("b_date_time", 6), "LtEq", column("expires", 2)))
+    filt = coalesce_batches_exec(filter_exec(between, join))
+    mx = aggregate_expr("max", "MAX(bid.price)", column("price", 5), "Int32")
+    inner = two_phase_aggregate([("a_id", 0)], [mx], filt, n)                              # a_id, MAX(bid.price)
+    q = projection_exec([(column("a_id", 0), "id"), (column("MAX(bid.price)", 1), "final")], inner)
+    bid = repartition_rr(memory_exec(BID, [0, 1, 2, 3]), n)
+    lsh2 = coalesce_batches_exec(repartition_hash(bid, [column("auction", 0), column("price", 2)], n))
+    rsh2 = coalesce_batches_exec(repartition_hash(q, [column("id", 0), column("final", 1)], n))
+    outer = hash_join_exec(lsh2, rsh2, [(column("auction", 0), column("id", 0)), (column("price", 2), column("final", 1))])
+    return projection_exec([(column("auction", 0), "auction"), (column("bidder", 1), "bidder"), (column("price", 2), "price"),
+                            (column("b_date_time", 3), "b_date_time")], coalesce_batches_exec(outer))
+
+
+def q12(n: int = TARGET_PARTITIONS) -> dict:
+    """benchmarks/src/nexmark/query/q12.sql, types q12_plan.fmt: SELECT bidder, COUNT(*) AS bid_count, MIN(p_time) AS
+    start_time, MAX(p_time) AS end_time FROM bid GROUP BY bidder, over bids that carry a processing time p_time."""
+    scan = repartition_rr(memory_exec(BID_PTIME, [1, 4]), n)          # bidder, p_time
+    cnt = aggregate_expr("count", "COUNT(UInt8(1))", literal("UInt8", 1), "UInt64")
+    mn = aggregate_expr("min", "MIN(bid.p_time)", column("p_time", 1), TS_NS_UTC)
+    mx = aggregate_expr("max", "MAX(bid.p_time)", column("p_time", 1), TS_NS_UTC)
+    agg = two_phase_aggregate([("bidder", 0)], [cnt, mn, mx], scan, n)
+    return projection_exec([(column("bidder", 0), "bidder"), (column("COUNT(UInt8(1))", 1), "bid_count"),
+                            (column("MIN(bid.p_time)", 2), "start_time"), (column("MAX(bid.p_time)", 3), "end_time")], agg)
+
+
+def q13(n: int = TARGET_PARTITIONS) -> dict:
+    """benchmarks/src/nexmark/query/q13.sql, types q13_plan.fmt:
+       SELECT auction, bidder, price, b_date_time, value FROM bid JOIN side_input ON auction = key"""
+    bid = repartition_rr(memory_exec(BID, [0, 1, 2, 3]), n)
+    side = repartition_rr(memory_exec(SIDE_INPUT, [0, 1]), n)
+    lsh = coalesce_batches_exec(repartition_hash(bid, [column("auction", 0)], n))
+    rsh = coalesce_batches_exec(repartition_hash(side, [column("key", 0)], n))
+    join = hash_join_exec(lsh, rsh, [(column("auction", 0), column("key", 0))])
+    # auction 0, bidder 1, price 2, b_date_time 3, key 4, value 5
+    return projection_exec([(column("auction", 0), "auction"), (column("bidder", 1), "bidder"), (column("price", 2), "price"),
+                            (column("b_date_time", 3), "b_date_time"), (column("value", 5), "value")], coalesce_batches_exec(join))
+
+
 QUERIES = {"q1": q1, "q2": q2, "q3": q3, "q4": q4, "q5": q5, "q6": q6, "q7": q7, "q8": q8}
 GPU_QUERIES = list(QUERIES)
 # relations each query feeds, in feed order (flock/src/datasource/nexmark/nexmark.rs:181-203); q5 scans bid
 # twice, and feed_data_sources hands one source to one leaf (context.rs:293-303), so bid is fed twice.
 SOURCES = {"q1": ["bid"], "q2": ["bid"], "q3": ["auction", "person"], "q4": ["auction", "bid"], "q5": ["bid", "bid"],
            "q6": ["auction", "bid"], "q7": ["bid", "bid"], "q8": ["person", "auction"]}
+# q9 / q10 / q12 / q13: kept apart from QUERIES, whose every entry the existing suites and bench.py iterate.
+# "bid_ptime" is nexgen.bids_ptime, "side_input" nexgen.side_input.
+MORE_QUERIES = {"q9": q9, "q10": q10, "q12": q12, "q13": q13}
+MORE_SOURCES = {"q9": ["auction", "bid", "bid"], "q10": ["bid"], "q12": ["bid_ptime"], "q13": ["bid", "side_input"]}
