@@ -282,8 +282,9 @@ TablePtr ProjectionExec::execute(const ExecEnv& env) {
 
 std::string FilterExec::fmt_as() const { return "FilterExec: " + expr_display(*predicate); }
 
-TablePtr FilterExec::execute(const ExecEnv& env) {
-  TablePtr in = input->execute(env);
+TablePtr FilterExec::execute(const ExecEnv& env) { return apply(env, input->execute(env)); }
+
+TablePtr FilterExec::apply(const ExecEnv& env, const TablePtr& in) const {
   Expr pred;
   emit_expr(*predicate, *in, &pred);
   return fg::filter_project(env.ctx, in, &pred, {}, {});
@@ -412,6 +413,91 @@ TablePtr HashAggregateExec::execute(const ExecEnv& env) {
   return result;
 }
 
+static ExecutionPlan* skip_to_operator(ExecutionPlan* p) {  // single GPU: repartitioning moves nothing either
+  while (true) {
+    p = skip_passthrough(p);
+    if (auto* r = dynamic_cast<RepartitionExec*>(p)) { p = r->input.get(); continue; }
+    return p;
+  }
+}
+
+// ---- single GPU: COUNT(*) of an inner join grouped by columns of a small dimension (YSB) is one pass over the fact
+// relation (dim_count.cu).  `agg` is the aggregate evaluated over the join: the Partial itself, or the Partial below a
+// fused Final.  Returns {} when the plan has another shape (nothing executed yet).  Otherwise the join's inputs have
+// run, and the result holds either the counts (`counted`: group columns, then one UInt64 column per name of
+// `count_names`) or, when the executed inputs do not qualify, the join's output for the generic aggregate (`joined`):
+// no subtree runs twice.
+struct JoinCount {
+  TablePtr counted, joined;
+};
+
+static JoinCount join_count(const ExecEnv& env, const HashAggregateExec& agg, const std::vector<std::string>& count_names) {
+  if (env.world != 1 || agg.aggr_expr.empty() || agg.group_expr.empty()) return {};
+  for (const auto& a : agg.aggr_expr)
+    if (a.func != FLOCKGPU_AGG_COUNT || (a.expr && is_column_expr(*a.expr))) return {};  // COUNT(*) only
+  for (const auto& g : agg.group_expr)
+    if (!is_column_expr(*g.first)) return {};
+  auto* join = dynamic_cast<HashJoinExec*>(skip_to_operator(agg.input.get()));
+  if (!join || join->on.size() != 1) return {};
+  // a FilterExec below a join input (through pass-throughs) hands over its input: its predicate may move into the kernel
+  TablePtr in[2];
+  FilterExec* filter[2] = {};
+  const PlanPtr* child[2] = {&join->left, &join->right};
+  for (int i = 0; i < 2; ++i) {
+    filter[i] = dynamic_cast<FilterExec*>(skip_to_operator(child[i]->get()));
+    in[i] = filter[i] ? filter[i]->input->execute(env) : (*child[i])->execute(env);
+    in[i]->resolve();
+  }
+  auto generic = [&] {
+    for (int i = 0; i < 2; ++i)
+      if (filter[i]) in[i] = filter[i]->apply(env, in[i]);
+    return JoinCount{nullptr, join->join(env, in[0], in[1])};
+  };
+  // every group column must come from one side, the dimension (a filter keeps its input's columns)
+  fg::Table joined_cols;
+  for (int i = 0; i < 2; ++i)
+    for (const fg::Column& c : in[i]->cols) joined_cols.cols.push_back(c);
+  const int n_left = int(in[0]->cols.size());
+  int dim = -1;
+  std::vector<int> group_cols;
+  for (const auto& g : agg.group_expr) {
+    const int c = column_of(*g.first, joined_cols);
+    const int side = c < n_left ? 0 : 1;
+    if (dim >= 0 && side != dim) return generic();
+    dim = side;
+    group_cols.push_back(c - (side ? n_left : 0));
+  }
+  const int fact = 1 - dim;
+  const int key[2] = {resolve_column(*in[0], join->on[0].first.name, join->on[0].first.index),
+                      resolve_column(*in[1], join->on[0].second.name, join->on[0].second.index)};
+  const fg::Column& fk = in[fact]->cols[key[fact]];
+  const fg::Column& dk = in[dim]->cols[key[dim]];
+  bool ok = fk.dtype == dk.dtype && fg::dim_count_key_type(fk.dtype) && !fk.all_null && !dk.all_null && in[fact]->cols.size() <= size_t(fg::MAX_IN_COLS);
+  for (int g : group_cols) ok &= !in[dim]->cols[g].all_null;
+  for (const fg::Column& c : in[fact]->cols) ok &= !c.all_null;
+  if (!ok) return generic();
+  if (filter[dim]) {
+    in[dim] = filter[dim]->apply(env, in[dim]);
+    filter[dim] = nullptr;
+  }
+  in[dim]->resolve();
+  if (in[dim]->num_rows > fg::DIM_COUNT_MAX_ROWS) return generic();
+  Expr pred;
+  if (filter[fact]) {
+    emit_expr(*filter[fact]->predicate, *in[fact], &pred);
+    std::vector<fg::ColInfo> infos;
+    for (const fg::Column& c : in[fact]->cols) infos.push_back({c.dtype, c.name, c.format, c.validity != nullptr});
+    if (fg::compile_predicate(pred, infos).prog.has_div_by_col) {  // the filter reports a division by zero itself
+      in[fact] = filter[fact]->apply(env, in[fact]);
+      filter[fact] = nullptr;
+    }
+  }
+  // the join's output carries the left input's schema metadata, and so does an aggregate over it
+  return JoinCount{fg::dim_count_aggregate(env.ctx, in[fact], key[fact], filter[fact] ? &pred : nullptr, in[dim], key[dim], group_cols, count_names,
+                                           in[0]->metadata),
+                   nullptr};
+}
+
 TablePtr HashAggregateExec::execute_uncached(const ExecEnv& env) {
   const bool final_mode = mode == FLOCKGPU_AGG_FINAL || mode == FLOCKGPU_AGG_FINAL_PARTITIONED;
   // ---- single-GPU fusion: Final*( Coalesce/Repartition ( Partial(x) ) ) == one SINGLE aggregate over x
@@ -424,7 +510,12 @@ TablePtr HashAggregateExec::execute_uncached(const ExecEnv& env) {
     }
     if (auto* partial = dynamic_cast<HashAggregateExec*>(p)) {
       if (partial->mode == FLOCKGPU_AGG_PARTIAL && partial->group_expr.size() == group_expr.size() && partial->aggr_expr.size() == aggr_expr.size()) {
-        TablePtr in = partial->input->execute(env);
+        std::vector<std::string> count_names, group_names;
+        for (const auto& a : aggr_expr) count_names.push_back(a.name);
+        for (const auto& g : group_expr) group_names.push_back(g.second);
+        JoinCount jc = join_count(env, *partial, count_names);
+        if (jc.counted) return rename_columns(env, jc.counted, group_names);
+        TablePtr in = jc.joined ? jc.joined : partial->input->execute(env);
         std::vector<int> gcols = group_columns(*partial, *in);
         std::vector<fg::AggSpec> specs;
         for (size_t i = 0; i < partial->aggr_expr.size(); ++i) {
@@ -440,7 +531,15 @@ TablePtr HashAggregateExec::execute_uncached(const ExecEnv& env) {
       }
     }
   }
-  TablePtr in = input->execute(env);
+  JoinCount jc;
+  if (mode == FLOCKGPU_AGG_PARTIAL) {
+    std::vector<std::string> count_names, group_names;
+    for (const auto& a : aggr_expr) count_names.push_back(a.name + "[count]");
+    for (const auto& g : group_expr) group_names.push_back(g.second);
+    jc = join_count(env, *this, count_names);
+    if (jc.counted) return rename_columns(env, jc.counted, group_names);
+  }
+  TablePtr in = jc.joined ? jc.joined : input->execute(env);
   std::vector<int> gcols = group_columns(*this, *in);
   // A Partial DISTINCT (no aggregate functions) ahead of a shuffle only exists to shrink what travels.  With Utf8 / wide
   // group keys it costs a full row-representative hash table (q8: 2.5 M persons that are all different), so
@@ -498,9 +597,9 @@ std::string HashJoinExec::fmt_as() const {
   return s + "]";
 }
 
-TablePtr HashJoinExec::execute(const ExecEnv& env) {
-  TablePtr l = left->execute(env);
-  TablePtr r = right->execute(env);
+TablePtr HashJoinExec::execute(const ExecEnv& env) { return join(env, left->execute(env), right->execute(env)); }
+
+TablePtr HashJoinExec::join(const ExecEnv& env, const TablePtr& l, const TablePtr& r) const {
   std::vector<int> lk, rk;
   for (const auto& p : on) {
     lk.push_back(resolve_column(*l, p.first.name, p.first.index));

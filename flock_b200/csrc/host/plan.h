@@ -95,6 +95,7 @@ class FilterExec : public UnaryExec {
   const char* name() const override { return "FilterExec"; }
   std::string fmt_as() const override;
   TablePtr execute(const ExecEnv& env) override;
+  TablePtr apply(const ExecEnv& env, const TablePtr& in) const;  // the filter over its already executed input
 };
 
 class CoalesceBatchesExec : public UnaryExec {
@@ -152,6 +153,7 @@ class HashJoinExec : public ExecutionPlan {
   std::vector<PlanPtr> children() const override { return {left, right}; }
   std::string fmt_as() const override;
   TablePtr execute(const ExecEnv& env) override;
+  TablePtr join(const ExecEnv& env, const TablePtr& l, const TablePtr& r) const;  // over already executed inputs
 };
 
 class SortExec : public UnaryExec {

@@ -508,6 +508,15 @@ TablePtr hash_aggregate(const CtxPtr& ctx, const TablePtr& in, int mode, const s
 double distinct_sample_duplicates(const CtxPtr& ctx, const TablePtr& in, const std::vector<int>& group_cols);
 TablePtr hash_join(const CtxPtr& ctx, const TablePtr& left, const TablePtr& right,
                    const std::vector<int>& left_keys, const std::vector<int>& right_keys);
+// COUNT(*) of `fact JOIN dim ON fact.fact_key = dim.dim_key` (inner) [WHERE `predicate` over the fact's columns],
+// grouped by the dimension's `group_cols`, in one pass over the fact (dim_count.cu).  Output: the group columns under
+// their dimension names, then one UInt64 count column per name of `count_names` (COUNT(*) listed n times: n equal
+// columns); schema metadata `metadata`.  The dimension holds at most
+// DIM_COUNT_MAX_ROWS rows: its key table (2 slots per row) and one counter per row fill 48 KiB of shared memory.
+constexpr int64_t DIM_COUNT_MAX_ROWS = 4096;
+bool dim_count_key_type(int dtype);  // Int32, Int64, UInt64, Timestamp, Utf8
+TablePtr dim_count_aggregate(const CtxPtr& ctx, const TablePtr& fact, int fact_key, const Expr* predicate, const TablePtr& dim, int dim_key,
+                             const std::vector<int>& group_cols, const std::vector<std::string>& count_names, const std::string& metadata);
 std::vector<TablePtr> hash_partition(const CtxPtr& ctx, const TablePtr& in, const std::vector<int>& keys,
                                      int n_parts);
 // The columns of `keys` that actually route a row: the fixed-width ones when there are any (hashing `p_id` routes

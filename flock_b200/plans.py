@@ -11,7 +11,7 @@ from __future__ import annotations
 
 import pyarrow as pa
 
-from . import nexgen
+from . import nexgen, ysbgen
 
 TARGET_PARTITIONS = 8     # flock/src/configs/flock.toml:113
 TARGET_BATCH_SIZE = 4096  # CoalesceBatchesExec default seen in every plan dump
@@ -356,3 +356,55 @@ SOURCES = {"q1": ["bid"], "q2": ["bid"], "q3": ["auction", "person"], "q4": ["au
 # "bid_ptime" is nexgen.bids_ptime, "side_input" nexgen.side_input.
 MORE_QUERIES = {"q9": q9, "q10": q10, "q12": q12, "q13": q13}
 MORE_SOURCES = {"q9": ["auction", "bid", "bid"], "q10": ["bid"], "q12": ["bid_ptime"], "q13": ["bid", "side_input"]}
+
+
+# ---- YSB, the Yahoo Streaming Benchmark (benchmarks/src/ysb/ysb.sql) --------------------------------------------------
+AD_EVENT, CAMPAIGN = ysbgen.ad_event_schema(), ysbgen.campaign_schema()
+YSB_COUNT = "COUNT(UInt8(1))"
+
+
+def _ysb_count() -> dict:
+    return aggregate_expr("count", YSB_COUNT, literal("UInt8", 1), "UInt64")
+
+
+def ysb_stage0(n: int = TARGET_PARTITIONS) -> list[dict]:
+    """planner.rs:315-327: the two shuffling plans, the viewed events by ad_id and the campaigns by c_ad_id."""
+    scan = repartition_rr(memory_exec(AD_EVENT, [2, 4]), n)                               # ad_id, event_type
+    views = coalesce_batches_exec(filter_exec(binary(column("event_type", 1), "Eq", literal("Utf8", "view")), scan))
+    events = coalesce_batches_exec(repartition_hash(views, [column("ad_id", 0)], n))
+    camps = coalesce_batches_exec(repartition_hash(repartition_rr(memory_exec(CAMPAIGN, [0, 1]), n), [column("c_ad_id", 0)], n))
+    return [events, camps]
+
+
+def _ysb_partial(events: dict, camps: dict) -> dict:
+    # ad_id 0, event_type 1, c_ad_id 2, campaign_id 3
+    join = coalesce_batches_exec(hash_join_exec(events, camps, [(column("ad_id", 0), column("c_ad_id", 0))]))
+    return hash_aggregate_exec("Partial", [(column("campaign_id", 3), "campaign_id")], [_ysb_count()], join)
+
+
+def _ysb_final(input: dict) -> dict:
+    final = hash_aggregate_exec("FinalPartitioned", [(column("campaign_id", 0), "campaign_id")], [_ysb_count()], input)
+    return projection_exec([(column("campaign_id", 0), "campaign_id"), (column(YSB_COUNT, 1), YSB_COUNT)], final)
+
+
+def ysb_stages(n: int = TARGET_PARTITIONS) -> list[list[dict]]:
+    """planner.rs:315-345: the query stages a distributed run hands to its functions, in order.  Stage 1 reads the
+    outputs of stage 0 (viewed events, campaigns), stage 2 the output of stage 1 (campaign_id and the COUNT state)."""
+    views = pa.schema([AD_EVENT.field("ad_id"), AD_EVENT.field("event_type")], metadata=AD_EVENT.metadata)
+    partial = _ysb_partial(memory_exec(views, None), memory_exec(CAMPAIGN, None))
+    stage1 = coalesce_batches_exec(repartition_hash(partial, [column("campaign_id", 0)], n))
+    states = pa.schema([pa.field("campaign_id", pa.utf8(), False), pa.field(YSB_COUNT + "[count]", pa.uint64(), True)], metadata=AD_EVENT.metadata)
+    return [ysb_stage0(n), [stage1], [_ysb_final(memory_exec(states, None))]]
+
+
+def ysb(n: int = TARGET_PARTITIONS) -> dict:
+    """SELECT campaign_id, COUNT(*) FROM ad_event INNER JOIN campaign ON ad_id = c_ad_id WHERE event_type = 'view'
+       GROUP BY campaign_id
+    as ONE plan, the three stages of planner.rs:315-345 stacked (centralized mode runs the whole plan in one worker)."""
+    events, camps = ysb_stage0(n)
+    shuffled = coalesce_batches_exec(repartition_hash(_ysb_partial(events, camps), [column("campaign_id", 0)], n))
+    return _ysb_final(shuffled)
+
+
+YSB_QUERIES = {"ysb": ysb}
+YSB_SOURCES = {"ysb": ["ad_event", "campaign"]}
