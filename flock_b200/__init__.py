@@ -21,7 +21,7 @@ import pyarrow as pa
 from . import _ffi
 from ._ffi import FlockGpuError, lib, check
 
-__all__ = ["Context", "Table", "HostRelation", "ExecutionContext", "Window", "FlockGpuError", "col", "lit", "E"]
+__all__ = ["Context", "Table", "HostRelation", "ExecutionContext", "Window", "FlockGpuError", "col", "lit", "null", "case", "E"]
 
 # enum flockgpu_dtype
 BOOL, INT32, INT64, UINT64, FLOAT64, TIMESTAMP, UTF8, UINT32 = range(8)
@@ -33,6 +33,8 @@ OP_COLUMN, OP_LIT_I64, OP_LIT_F64, OP_LIT_UTF8, OP_CAST = 1, 2, 3, 4, 5
 OP_ADD, OP_SUB, OP_MUL, OP_DIV, OP_MOD = 10, 11, 12, 13, 14
 OP_EQ, OP_NE, OP_LT, OP_LE, OP_GT, OP_GE = 20, 21, 22, 23, 24, 25
 OP_AND, OP_OR, OP_NOT = 30, 31, 32
+OP_NEG, OP_IS_NULL, OP_IS_NOT_NULL, OP_LIT_NULL, OP_CASE, OP_IN_LIST = 40, 41, 42, 43, 44, 45
+CASE_HAS_BASE, CASE_HAS_ELSE = 1, 2
 # enum flockgpu_agg_mode / flockgpu_agg_func
 AGG_PARTIAL, AGG_FINAL, AGG_FINAL_PARTITIONED, AGG_SINGLE = 0, 1, 2, 3
 AGG_COUNT, AGG_SUM, AGG_MIN, AGG_MAX, AGG_AVG = 0, 1, 2, 3, 4
@@ -84,6 +86,17 @@ class E:
     def __and__(self, o): return self._bin(OP_AND, o)
     def __or__(self, o): return self._bin(OP_OR, o)
     def __invert__(self): return E(self.tokens + [(OP_NOT, 0, 0, 0, 0.0, None)])
+    def __neg__(self): return E(self.tokens + [(OP_NEG, 0, 0, 0, 0.0, None)])
+    def is_null(self) -> "E": return E(self.tokens + [(OP_IS_NULL, 0, 0, 0, 0.0, None)])
+    def is_not_null(self) -> "E": return E(self.tokens + [(OP_IS_NOT_NULL, 0, 0, 0, 0.0, None)])
+
+    def isin(self, values, negated: bool = False) -> "E":
+        """self [NOT] IN (values): literals (None = a NULL literal)."""
+        toks = list(self.tokens)
+        for v in values:
+            toks += (null() if v is None else E.wrap(v)).tokens
+        return E(toks + [(OP_IN_LIST, 0, 1 if negated else 0, len(values), 0.0, None)])
+
     __hash__ = None
 
 
@@ -102,6 +115,22 @@ def lit(value, dtype: str | None = None) -> E:
     if isinstance(value, str):
         return E([(OP_LIT_UTF8, UTF8, 0, 0, 0.0, value.encode("utf-8"))])
     raise TypeError(f"unsupported literal {value!r}")
+
+
+def null(dtype: str = "int64") -> E:
+    """A NULL literal of the given type."""
+    return E([(OP_LIT_NULL, _DTYPE_BY_NAME[dtype], 0, 0, 0.0, None)])
+
+
+def case(when_then, otherwise=None, base=None) -> E:
+    """CASE [base] WHEN w THEN t ... [ELSE otherwise] END; `when_then` is a list of (when, then) pairs."""
+    toks = [] if base is None else list(E.wrap(base).tokens)
+    for w, t in when_then:
+        toks += E.wrap(w).tokens + E.wrap(t).tokens
+    if otherwise is not None:
+        toks += E.wrap(otherwise).tokens
+    flags = (CASE_HAS_BASE if base is not None else 0) | (CASE_HAS_ELSE if otherwise is not None else 0)
+    return E(toks + [(OP_CASE, 0, flags, len(when_then), 0.0, None)])
 
 
 class _CExpr:
@@ -547,6 +576,35 @@ def selftest_eval_predicate(batch: pa.RecordBatch, predicate: E):
     finally:
         _release_exported(c_schema, arrays, 1)
     return mask[:batch.num_rows].astype(bool), fast.value
+
+
+def selftest_eval_tree(batch: pa.RecordBatch, exprs, predicate: bool = False):
+    """CPU-only check of the TREE form (flockgpu_selftest_eval_tree): all of `exprs` compiled into one register program
+    and run by the kernels' interpreter on the host.  predicate=True: `exprs` is one predicate, returns (bool mask,
+    instruction count).  Otherwise returns ([(values | None for a plain column, valid mask, dtype)], instruction count)."""
+    import numpy as np
+    single = isinstance(exprs, E)
+    es = [_CExpr(E.wrap(e)) for e in ([exprs] if single else exprs)]
+    n, k = batch.num_rows, len(es)
+    arr = (_ffi.Expr * k)(*[e.expr for e in es])
+    vals = [np.zeros(max(n, 1), np.int64) for _ in range(k)]
+    valid = [np.ones(max(n, 1), np.uint8) for _ in range(k)]
+    pv = (C.c_void_p * k)(*[v.ctypes.data for v in vals])
+    pm = (C.c_void_p * k)(*[v.ctypes.data for v in valid])
+    dts, passes, n_instr = (C.c_int32 * k)(), (C.c_int32 * k)(), C.c_int32()
+    c_schema, arrays, ptrs = _export_batches(batch.schema, [batch])
+    try:
+        check(lib.flockgpu_selftest_eval_tree(C.byref(c_schema), ptrs[0], arr, k, 1 if predicate else 0, pv, pm, dts, passes, C.byref(n_instr)))
+    finally:
+        _release_exported(c_schema, arrays, 1)
+    if predicate:
+        return vals[0].view(np.uint8)[:n].astype(bool), n_instr.value
+    views = {INT32: np.int32, UINT32: np.uint32, FLOAT64: np.float64, UINT64: np.uint64}
+    out = []
+    for i in range(k):
+        v = None if passes[i] else vals[i].view(views.get(dts[i], np.int64))[:n].copy()
+        out.append((v, valid[i][:n].astype(bool), dts[i]))
+    return out, n_instr.value
 
 
 def selftest_zstd_decompress(data: bytes, capacity: int) -> bytes:

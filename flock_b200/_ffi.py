@@ -170,6 +170,7 @@ PROTOTYPES = {
     "flock_context_plan_str": (C.c_char_p, [_P, C.c_int32]),
     "flockgpu_selftest_eval_predicate": (C.c_int, [C.POINTER(ArrowSchema), C.POINTER(ArrowArray), C.POINTER(Expr), _P, _I32P]),
     "flockgpu_selftest_eval_value": (C.c_int, [C.POINTER(ArrowSchema), C.POINTER(ArrowArray), C.POINTER(Expr), _P, _I32P, _I32P]),
+    "flockgpu_selftest_eval_tree": (C.c_int, [C.POINTER(ArrowSchema), C.POINTER(ArrowArray), C.POINTER(Expr), C.c_int32, C.c_int32, _PP, _PP, _I32P, _I32P, _I32P]),
     "flockgpu_selftest_zstd_decompress": (C.c_int, [_P, C.c_int64, _P, C.c_int64, C.POINTER(C.c_int64)]),
     "flockgpu_selftest_zstd_compress": (C.c_int, [_P, C.c_int64, _P, C.c_int64, C.POINTER(C.c_int64)]),
     "flockgpu_selftest_pred_i32": (C.c_int, [C.c_int64, C.c_int32, C.c_int64, _I32P, C.c_int64, C.POINTER(C.c_uint8), _I32P]),

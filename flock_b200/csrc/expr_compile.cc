@@ -8,9 +8,12 @@
 // casts, the usual numeric promotion (Float64 > 64-bit ints > Int32) is applied.
 #include "expr_compile.h"
 
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <functional>
+#include <map>
+#include <set>
 
 namespace fg {
 
@@ -24,6 +27,8 @@ struct Node {
   double d = 0;
   std::string s;
   int l = -1, r = -1;
+  std::vector<int> kids;  // CASE: [base] (when, then)... [else]; IN_LIST: value, literals...
+  int flags = 0;          // CASE: FLOCKGPU_CASE_HAS_*; IN_LIST: 1 = NOT IN
 };
 
 bool is_arith(int op) { return op >= FLOCKGPU_OP_ADD && op <= FLOCKGPU_OP_MOD; }
@@ -99,6 +104,73 @@ Tree build_tree(const Expr& e, const std::vector<ColInfo>& cols) {
         n.dtype = FLOCKGPU_BOOL;
         FG_CHECK(t.nodes[n.l].dtype == FLOCKGPU_BOOL, FLOCKGPU_ERR_INVALID, "expression: NOT of a non-boolean");
         break;
+      case FLOCKGPU_OP_LIT_NULL:
+        FG_CHECK(tok.dtype >= FLOCKGPU_BOOL && tok.dtype <= FLOCKGPU_UINT32, FLOCKGPU_ERR_INVALID, "expression: NULL literal of unknown type %d", tok.dtype);
+        n.dtype = tok.dtype;
+        break;
+      case FLOCKGPU_OP_NEG:
+        n.l = pop();
+        n.dtype = t.nodes[n.l].dtype;
+        FG_CHECK(is_numeric(n.dtype) && !is_unsigned(n.dtype), FLOCKGPU_ERR_UNSUPPORTED, "expression: unary minus on %s", dtype_name(n.dtype));
+        break;
+      case FLOCKGPU_OP_IS_NULL:
+      case FLOCKGPU_OP_IS_NOT_NULL:
+        n.l = pop();
+        n.dtype = FLOCKGPU_BOOL;
+        break;
+      case FLOCKGPU_OP_CASE: {
+        n.flags = tok.col;
+        const bool has_base = tok.col & FLOCKGPU_CASE_HAS_BASE, has_else = tok.col & FLOCKGPU_CASE_HAS_ELSE;
+        FG_CHECK(tok.i64 >= 1 && tok.i64 <= 64 && (tok.col & ~3) == 0, FLOCKGPU_ERR_INVALID, "expression: malformed CASE (%lld WHEN branches, flags %d)",
+                 (long long)tok.i64, tok.col);
+        const size_t need = size_t(2 * tok.i64) + has_base + has_else;
+        FG_CHECK(stack.size() >= need, FLOCKGPU_ERR_INVALID, "expression: CASE needs %zu operands, %zu on the stack (malformed postfix program)", need,
+                 stack.size());
+        n.kids.assign(stack.end() - need, stack.end());
+        stack.resize(stack.size() - need);
+        // result type: the common type of the THEN / ELSE values that are not NULL literals
+        int dt = -1;
+        for (size_t k = has_base ? 1 : 0; k < n.kids.size(); ++k) {
+          const bool is_value = k + 1 == n.kids.size() && has_else ? true : ((k - (has_base ? 1 : 0)) & 1) == 1;
+          const Node& c = t.nodes[n.kids[k]];
+          if (!is_value) {
+            if (has_base) {
+              const int bt = t.nodes[n.kids[0]].dtype;
+              FG_CHECK((is_numeric(bt) && is_numeric(c.dtype)) || (bt == FLOCKGPU_UTF8 && c.dtype == FLOCKGPU_UTF8), FLOCKGPU_ERR_UNSUPPORTED,
+                       "expression: CASE compares %s with %s", dtype_name(bt), dtype_name(c.dtype));
+            } else {
+              FG_CHECK(c.dtype == FLOCKGPU_BOOL, FLOCKGPU_ERR_INVALID, "expression: CASE WHEN condition is not boolean");
+            }
+            continue;
+          }
+          if (c.op == FLOCKGPU_OP_LIT_NULL) continue;
+          if (dt < 0) dt = c.dtype;
+          else if (is_numeric(dt) && is_numeric(c.dtype)) dt = promote(dt, c.dtype);
+          else FG_CHECK(dt == c.dtype, FLOCKGPU_ERR_INVALID, "expression: CASE branches of types %s and %s", dtype_name(dt), dtype_name(c.dtype));
+        }
+        if (dt < 0) dt = t.nodes[n.kids.back()].dtype;  // every branch is a NULL literal
+        n.dtype = dt;
+        break;
+      }
+      case FLOCKGPU_OP_IN_LIST: {
+        n.flags = tok.col;
+        FG_CHECK(tok.i64 >= 1 && tok.i64 <= 64 && (tok.col & ~1) == 0, FLOCKGPU_ERR_INVALID, "expression: malformed IN list (%lld literals, flags %d)",
+                 (long long)tok.i64, tok.col);
+        const size_t need = size_t(tok.i64) + 1;
+        FG_CHECK(stack.size() >= need, FLOCKGPU_ERR_INVALID, "expression: IN list needs %zu operands, %zu on the stack (malformed postfix program)", need,
+                 stack.size());
+        n.kids.assign(stack.end() - need, stack.end());
+        stack.resize(stack.size() - need);
+        const int vt = t.nodes[n.kids[0]].dtype;
+        for (size_t k = 1; k < n.kids.size(); ++k) {
+          const Node& c = t.nodes[n.kids[k]];
+          FG_CHECK(is_literal(c) || c.op == FLOCKGPU_OP_LIT_NULL, FLOCKGPU_ERR_INVALID, "expression: IN list entry %zu is not a literal", k - 1);
+          FG_CHECK(c.op == FLOCKGPU_OP_LIT_NULL || (is_numeric(vt) && is_numeric(c.dtype)) || (vt == FLOCKGPU_UTF8 && c.dtype == FLOCKGPU_UTF8),
+                   FLOCKGPU_ERR_UNSUPPORTED, "expression: %s IN a list with a %s literal", dtype_name(vt), dtype_name(c.dtype));
+        }
+        n.dtype = FLOCKGPU_BOOL;
+        break;
+      }
       default:
         if (is_arith(tok.op) || is_cmp(tok.op) || tok.op == FLOCKGPU_OP_AND || tok.op == FLOCKGPU_OP_OR) {
           n.r = pop();
@@ -539,6 +611,358 @@ CompiledPredicate compile_predicate(const Expr& e, const std::vector<ColInfo>& c
   return out;
 }
 
+// ------------------------------------------------------------------------------------------------
+// the tree form (expr_tree.h)
+// ------------------------------------------------------------------------------------------------
+namespace {
+
+// A value of the program before registers are assigned.  Nodes are hash-consed: the same operation over the same
+// operands is one node, across all the expressions of a program.
+struct TNode {
+  int op = 0, sub = 0;
+  int a = -1, b = -1, c = -1;  // operand nodes
+  int col = -1, col2 = -1;
+  Val lit{};
+  bool null_lit = false;
+  bool may_null = false;
+};
+
+struct TreeBuilder {
+  const std::vector<ColInfo>& cols;
+  std::vector<TNode> ir;
+  std::map<std::string, int> interned;
+  std::string pool;
+  bool may_fail = false;
+  explicit TreeBuilder(const std::vector<ColInfo>& c) : cols(c) {}
+
+  int intern(const TNode& n) {
+    char key[160];
+    snprintf(key, sizeof key, "%d.%d.%d.%d.%d.%d.%d.%llx.%d", n.op, n.sub, n.a, n.b, n.c, n.col, n.col2, (unsigned long long)n.lit.u, int(n.null_lit));
+    auto it = interned.find(key);
+    if (it != interned.end()) return it->second;
+    ir.push_back(n);
+    interned[key] = int(ir.size()) - 1;
+    return int(ir.size()) - 1;
+  }
+  bool nullable(int id) const { return id >= 0 && ir[id].may_null; }
+
+  int lit_node(Val v, bool is_null) {
+    TNode n;
+    n.op = T_LIT;
+    n.lit = is_null ? Val{0} : v;
+    n.null_lit = is_null;
+    n.may_null = is_null;
+    return intern(n);
+  }
+  int unary(int op, int sub, int a) {
+    TNode n;
+    n.op = op;
+    n.sub = sub;
+    n.a = a;
+    n.may_null = (op == T_IS_NULL || op == T_IS_NOT_NULL) ? false : nullable(a);
+    return intern(n);
+  }
+  int binary(int op, int sub, int a, int b) {
+    TNode n;
+    n.op = op;
+    n.sub = sub;
+    n.a = a;
+    n.b = b;
+    n.may_null = nullable(a) || nullable(b);
+    return intern(n);
+  }
+  int select(int cond, int a, int b) {
+    TNode n;
+    n.op = T_SELECT;
+    n.c = cond;
+    n.a = a;
+    n.b = b;
+    n.may_null = nullable(a) || nullable(b);
+    return intern(n);
+  }
+  // `id` (canonical form of `from`) converted to the canonical form of `to`: the steps ChainBuilder::convert pushes
+  int convert(int id, int from, int to) {
+    if (from == to || from == FLOCKGPU_BOOL || to == FLOCKGPU_BOOL) return id;
+    if (to == FLOCKGPU_FLOAT64) return unary(T_ARITH, is_unsigned(from) ? C_U2F : C_I2F, id);
+    if (from == FLOCKGPU_FLOAT64) id = unary(T_ARITH, C_F2I, id);
+    if (to == FLOCKGPU_INT32) return unary(T_ARITH, C_WRAP_I32, id);
+    if (to == FLOCKGPU_UINT32) return unary(T_ARITH, C_WRAP_U32, id);
+    return id;
+  }
+  int pooled(const std::string& s, Val* where) {
+    size_t at = pool.find(s);
+    if (at == std::string::npos || s.empty()) {
+      at = s.empty() ? 0 : pool.size();
+      if (!s.empty()) pool += s;
+    }
+    FG_CHECK(pool.size() <= size_t(TREE_POOL_BYTES), FLOCKGPU_ERR_UNSUPPORTED, "expression: Utf8 literals exceed %d bytes", TREE_POOL_BYTES);
+    where->u = (uint64_t(at) << 32) | uint64_t(s.size());
+    return 0;
+  }
+
+  // `l CMP r` over tree nodes li, ri
+  int compare(const Tree& t, int cmp, int li, int ri, std::vector<int>& memo) {
+    const Node& l = t.nodes[li];
+    const Node& r = t.nodes[ri];
+    if (l.op == FLOCKGPU_OP_LIT_NULL || r.op == FLOCKGPU_OP_LIT_NULL) return lit_node(Val{0}, true);  // x CMP NULL is NULL
+    if (l.dtype == FLOCKGPU_UTF8) {
+      const Node* colside = &l;
+      const Node* other = &r;
+      if (l.op != FLOCKGPU_OP_COLUMN) {
+        colside = &r;
+        other = &l;
+        cmp = swap_cmp(cmp);
+      }
+      FG_CHECK(colside->op == FLOCKGPU_OP_COLUMN, FLOCKGPU_ERR_UNSUPPORTED, "expression: Utf8 comparison needs a column operand");
+      TNode n;
+      n.op = T_CMP_UTF8;
+      n.sub = cmp;
+      n.col = colside->col;
+      n.may_null = cols[colside->col].has_nulls;
+      if (other->op == FLOCKGPU_OP_COLUMN) {
+        n.col2 = other->col;
+        n.may_null |= cols[other->col].has_nulls;
+      } else {
+        FG_CHECK(other->op == FLOCKGPU_OP_LIT_UTF8, FLOCKGPU_ERR_UNSUPPORTED, "expression: Utf8 comparison with a computed operand");
+        pooled(other->s, &n.lit);
+      }
+      return intern(n);
+    }
+    const int dom = cmp_domain(l.dtype, r.dtype);
+    int a = lower(t, li, memo), b = lower(t, ri, memo);
+    if (dom == DOM_F64) {
+      a = convert(a, l.dtype, FLOCKGPU_FLOAT64);
+      b = convert(b, r.dtype, FLOCKGPU_FLOAT64);
+    }
+    return binary(T_CMP, (dom << 8) | (cmp - FLOCKGPU_OP_EQ), a, b);
+  }
+
+  int lower(const Tree& t, int idx, std::vector<int>& memo) {
+    if (memo[idx] >= 0) return memo[idx];
+    const Node& n = t.nodes[idx];
+    int id = -1;
+    switch (n.op) {
+      case FLOCKGPU_OP_COLUMN: {
+        TNode x;
+        x.op = T_COL;
+        x.col = n.col;
+        x.may_null = cols[n.col].has_nulls;
+        id = intern(x);
+        break;
+      }
+      case FLOCKGPU_OP_LIT_I64:
+      case FLOCKGPU_OP_LIT_F64:
+        id = lit_node(literal_as(n, n.dtype), false);
+        break;
+      case FLOCKGPU_OP_LIT_NULL:
+        id = lit_node(Val{0}, true);
+        break;
+      case FLOCKGPU_OP_LIT_UTF8:
+        fail(FLOCKGPU_ERR_UNSUPPORTED, "expression: a Utf8 literal is only supported as a comparison operand or in an IN list");
+      case FLOCKGPU_OP_CAST:
+        FG_CHECK(t.nodes[n.l].dtype != FLOCKGPU_BOOL, FLOCKGPU_ERR_UNSUPPORTED, "expression: CAST of a boolean");
+        id = convert(lower(t, n.l, memo), t.nodes[n.l].dtype, n.dtype);
+        break;
+      case FLOCKGPU_OP_NEG:
+        if (n.dtype == FLOCKGPU_FLOAT64) {
+          Val m;
+          m.d = -1.0;  // x * -1 flips the sign of every value, zeros included, in one exact operation
+          id = binary(T_ARITH, C_MUL_F, lower(t, n.l, memo), lit_node(m, false));
+        } else {
+          id = binary(T_ARITH, C_RSUB_I, lower(t, n.l, memo), lit_node(Val{0}, false));
+          if (n.dtype == FLOCKGPU_INT32) id = unary(T_ARITH, C_WRAP_I32, id);
+        }
+        break;
+      case FLOCKGPU_OP_NOT:
+        id = unary(T_NOT, 0, lower(t, n.l, memo));
+        break;
+      case FLOCKGPU_OP_IS_NULL:
+      case FLOCKGPU_OP_IS_NOT_NULL: {
+        FG_CHECK(t.nodes[n.l].op != FLOCKGPU_OP_LIT_UTF8, FLOCKGPU_ERR_UNSUPPORTED, "expression: IS NULL of a Utf8 literal");
+        id = unary(n.op == FLOCKGPU_OP_IS_NULL ? T_IS_NULL : T_IS_NOT_NULL, 0, lower(t, n.l, memo));
+        break;
+      }
+      case FLOCKGPU_OP_AND:
+      case FLOCKGPU_OP_OR:
+        id = binary(n.op == FLOCKGPU_OP_AND ? T_AND : T_OR, 0, lower(t, n.l, memo), lower(t, n.r, memo));
+        break;
+      case FLOCKGPU_OP_CASE: {
+        FG_CHECK(n.dtype != FLOCKGPU_UTF8, FLOCKGPU_ERR_UNSUPPORTED, "expression: a CASE that returns Utf8 (computed Utf8 values are not supported)");
+        const bool has_base = n.flags & FLOCKGPU_CASE_HAS_BASE, has_else = n.flags & FLOCKGPU_CASE_HAS_ELSE;
+        const int first = has_base ? 1 : 0;
+        const int n_when = int(n.kids.size() - first - (has_else ? 1 : 0)) / 2;
+        auto value = [&](int kid) { return convert(lower(t, kid, memo), t.nodes[kid].dtype, n.dtype); };
+        id = has_else ? value(n.kids.back()) : lit_node(Val{0}, true);
+        for (int w = n_when - 1; w >= 0; --w) {
+          const int when = n.kids[first + 2 * w], then = n.kids[first + 2 * w + 1];
+          const int cond = has_base ? compare(t, FLOCKGPU_OP_EQ, n.kids[0], when, memo) : lower(t, when, memo);
+          id = select(cond, value(then), id);
+        }
+        break;
+      }
+      case FLOCKGPU_OP_IN_LIST: {
+        // x IN (a, b) is x = a OR x = b under Kleene's OR: exactly SQL's three-valued IN
+        for (size_t k = 1; k < n.kids.size(); ++k) {
+          const int eq = compare(t, FLOCKGPU_OP_EQ, n.kids[0], n.kids[k], memo);
+          id = id < 0 ? eq : binary(T_OR, 0, id, eq);
+        }
+        if (n.flags & 1) id = unary(T_NOT, 0, id);
+        break;
+      }
+      default:
+        if (is_cmp(n.op)) {
+          id = compare(t, n.op, n.l, n.r, memo);
+        } else {
+          FG_CHECK(is_arith(n.op), FLOCKGPU_ERR_INVALID, "expression: unknown opcode %d", n.op);
+          const int T = n.dtype;
+          const int a = convert(lower(t, n.l, memo), t.nodes[n.l].dtype, T);
+          const int b = convert(lower(t, n.r, memo), t.nodes[n.r].dtype, T);
+          id = binary(T_ARITH, ChainBuilder::arith_opcode(n.op, T, false), a, b);
+          if ((n.op == FLOCKGPU_OP_DIV || n.op == FLOCKGPU_OP_MOD) && T != FLOCKGPU_FLOAT64) may_fail = true;
+          if (T == FLOCKGPU_INT32) id = unary(T_ARITH, C_WRAP_I32, id);
+          if (T == FLOCKGPU_UINT32) id = unary(T_ARITH, C_WRAP_U32, id);
+        }
+    }
+    memo[idx] = id;
+    return id;
+  }
+
+  // Registers and instruction order: post-order from each root, a register freed at its value's last use.
+  // stores[k] >= 0: root k is written to output stores[k] as soon as it is computed.
+  void emit(const std::vector<int>& roots, const std::vector<int>& stores, bool predicate, CompiledTree* out) {
+    TreeProgram& p = out->prog;
+    memset(&p, 0, sizeof p);
+    p.result_reg = -1;
+    std::vector<int> uses(ir.size(), 0), reg(ir.size(), -1);
+    std::vector<char> seen(ir.size(), 0);
+    std::function<void(int)> count = [&](int id) {
+      if (id < 0) return;
+      ++uses[id];
+      if (seen[id]) return;
+      seen[id] = 1;
+      count(ir[id].a);
+      count(ir[id].b);
+      count(ir[id].c);
+    };
+    for (int r : roots) count(r);
+    // registers a node's subtree needs when it is evaluated on its own (operands are interned before their users)
+    std::vector<int> need(ir.size(), 1);
+    for (size_t id = 0; id < ir.size(); ++id) {
+      int k[3] = {ir[id].a < 0 ? 0 : need[ir[id].a], ir[id].b < 0 ? 0 : need[ir[id].b], ir[id].c < 0 ? 0 : need[ir[id].c]};
+      std::sort(k, k + 3, std::greater<int>());
+      need[id] = std::max({1, k[0], k[1] + (k[1] > 0), k[2] + 2 * (k[2] > 0)});
+    }
+    bool busy[TREE_REGS] = {};
+    std::set<int> cols_read;
+    auto push = [&](const TreeInstr& in) {
+      FG_CHECK(p.n_instr < TREE_MAX_INSTR, FLOCKGPU_ERR_UNSUPPORTED, "expression: the program needs more than %d instructions", TREE_MAX_INSTR);
+      p.ins[p.n_instr++] = in;
+    };
+    auto release = [&](int id) {
+      if (id >= 0 && --uses[id] == 0) busy[reg[id]] = false;
+    };
+    std::function<void(int)> gen = [&](int id) {
+      if (id < 0 || reg[id] >= 0) return;
+      const TNode& n = ir[id];
+      // the operand that needs the most registers first (Sethi-Ullman): the others' results are not held meanwhile
+      int kids[3] = {n.c, n.a, n.b};
+      std::stable_sort(kids, kids + 3, [&](int x, int y) { return (x < 0 ? 0 : need[x]) > (y < 0 ? 0 : need[y]); });
+      for (int k : kids) gen(k);
+      // the operands' last use may be this instruction: their registers are free for its result (every row reads its
+      // operands before it writes)
+      release(n.a);
+      release(n.b);
+      release(n.c);
+      int r = 0;
+      while (r < TREE_REGS && busy[r]) ++r;
+      FG_CHECK(r < TREE_REGS, FLOCKGPU_ERR_UNSUPPORTED, "expression: the tree needs more than %d registers at once", TREE_REGS);
+      busy[r] = true;
+      out->n_regs = std::max(out->n_regs, r + 1);
+      reg[id] = r;
+      TreeInstr in{};
+      in.op = int16_t(n.op);
+      in.sub = int16_t(n.sub);
+      in.d = int8_t(r);
+      in.a = int8_t(n.a >= 0 ? reg[n.a] : -1);
+      in.b = int8_t(n.b >= 0 ? reg[n.b] : -1);
+      in.c = int8_t(n.c >= 0 ? reg[n.c] : -1);
+      if (n.op == T_LIT) in.a = n.null_lit ? 1 : 0;
+      in.col = n.col;
+      in.col2 = n.col2;
+      in.lit = n.lit;
+      if (n.col >= 0) cols_read.insert(n.col);
+      if (n.col2 >= 0) cols_read.insert(n.col2);
+      push(in);
+    };
+    for (size_t k = 0; k < roots.size(); ++k) {
+      gen(roots[k]);
+      if (predicate) {
+        p.result_reg = reg[roots[k]];
+      } else {
+        TreeInstr st{};
+        st.op = T_STORE;
+        st.a = int8_t(reg[roots[k]]);
+        st.col = stores[k];
+        push(st);
+        release(roots[k]);
+      }
+    }
+    memcpy(p.pool, pool.data(), pool.size());
+    out->may_fail = may_fail;
+    out->cols_read.assign(cols_read.begin(), cols_read.end());
+  }
+};
+
+}  // namespace
+
+CompiledTree compile_tree_values(const std::vector<Expr>& exprs, const std::vector<ColInfo>& cols) {
+  CompiledTree out;
+  TreeBuilder b(cols);
+  std::vector<int> roots, stores;
+  for (const Expr& e : exprs) {
+    Tree t = build_tree(e, cols);
+    const Node& root = t.nodes[t.root];
+    TreeRoot r;
+    r.dtype = root.dtype;
+    FG_CHECK(root.dtype != FLOCKGPU_BOOL, FLOCKGPU_ERR_UNSUPPORTED, "projection: boolean-valued output columns are not supported");
+    if (root.op == FLOCKGPU_OP_COLUMN) {
+      r.passthrough = true;
+      r.src_col = root.col;
+      r.format = cols[root.col].format;
+    } else {
+      FG_CHECK(root.dtype != FLOCKGPU_UTF8, FLOCKGPU_ERR_UNSUPPORTED, "projection: computed Utf8 columns are not supported");
+      FG_CHECK(out.n_outs < TREE_MAX_OUTS, FLOCKGPU_ERR_UNSUPPORTED, "expression: more than %d computed values in one program", TREE_MAX_OUTS);
+      std::vector<int> memo(t.nodes.size(), -1);
+      const int id = b.lower(t, t.root, memo);
+      r.out = out.n_outs++;
+      r.may_be_null = b.ir[id].may_null;
+      r.format = default_format(root.dtype);
+      if (root.dtype == FLOCKGPU_TIMESTAMP)
+        for (const Node& n : t.nodes)
+          if (n.op == FLOCKGPU_OP_COLUMN && n.dtype == FLOCKGPU_TIMESTAMP) {
+            r.format = cols[n.col].format;
+            break;
+          }
+      roots.push_back(id);
+      stores.push_back(r.out);
+    }
+    out.roots.push_back(r);
+  }
+  b.emit(roots, stores, false, &out);
+  return out;
+}
+
+CompiledTree compile_tree_predicate(const Expr& e, const std::vector<ColInfo>& cols) {
+  CompiledTree out;
+  TreeBuilder b(cols);
+  Tree t = build_tree(e, cols);
+  FG_CHECK(t.nodes[t.root].dtype == FLOCKGPU_BOOL, FLOCKGPU_ERR_INVALID, "filter: predicate is not boolean");
+  std::vector<int> memo(t.nodes.size(), -1);
+  const int id = b.lower(t, t.root, memo);
+  b.emit({id}, {-1}, true, &out);
+  return out;
+}
+
 std::string expr_to_string(const Expr& e, const std::vector<ColInfo>& cols) {
   std::vector<std::string> st;
   auto opname = [](int op) -> const char* {
@@ -569,6 +993,38 @@ std::string expr_to_string(const Expr& e, const std::vector<ColInfo>& cols) {
         if (st.empty()) return "<malformed>";
         std::string a = st.back(); st.pop_back();
         st.push_back("NOT " + a);
+        break;
+      }
+      case FLOCKGPU_OP_LIT_NULL: st.push_back("NULL"); break;
+      case FLOCKGPU_OP_NEG:
+      case FLOCKGPU_OP_IS_NULL:
+      case FLOCKGPU_OP_IS_NOT_NULL: {
+        if (st.empty()) return "<malformed>";
+        std::string a = st.back(); st.pop_back();
+        st.push_back(t.op == FLOCKGPU_OP_NEG ? "(- " + a + ")" : a + (t.op == FLOCKGPU_OP_IS_NULL ? " IS NULL" : " IS NOT NULL"));
+        break;
+      }
+      case FLOCKGPU_OP_CASE: {
+        const bool has_base = t.col & FLOCKGPU_CASE_HAS_BASE, has_else = t.col & FLOCKGPU_CASE_HAS_ELSE;
+        const size_t need = size_t(2 * t.i64) + has_base + has_else;
+        if (t.i64 < 1 || st.size() < need) return "<malformed>";
+        const size_t at = st.size() - need;
+        std::string s = "CASE ";
+        if (has_base) s += st[at] + " ";
+        for (int64_t w = 0; w < t.i64; ++w) s += "WHEN " + st[at + has_base + 2 * w] + " THEN " + st[at + has_base + 2 * w + 1] + " ";
+        if (has_else) s += "ELSE " + st.back() + " ";
+        st.resize(at);
+        st.push_back(s + "END");
+        break;
+      }
+      case FLOCKGPU_OP_IN_LIST: {
+        const size_t need = size_t(t.i64) + 1;
+        if (t.i64 < 1 || st.size() < need) return "<malformed>";
+        const size_t at = st.size() - need;
+        std::string s = st[at] + (t.col ? " NOT IN ([" : " IN ([");
+        for (size_t k = 1; k < need; ++k) s += (k > 1 ? ", " : "") + st[at + k];
+        st.resize(at);
+        st.push_back(s + "])");
         break;
       }
       default: {

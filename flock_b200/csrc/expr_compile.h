@@ -5,6 +5,7 @@
 #include <vector>
 
 #include "expr_program.h"
+#include "expr_tree.h"
 #include "internal.h"
 
 namespace fg {
@@ -50,6 +51,32 @@ struct CompiledValue {
   int fast = FAST_VAL_NONE;
   double fast_lit = 0;
 };
+
+// The tree form (expr_tree.h): one register program for several value expressions, or for one predicate.
+struct TreeRoot {
+  bool passthrough = false;  // a plain column: nothing is computed
+  int src_col = -1;
+  int out = -1;              // computed: index of its TreeOut (T_STORE's `col`)
+  int dtype = FLOCKGPU_INT64;
+  std::string format;
+  bool may_be_null = false;  // computed: the result needs validity bytes
+};
+struct CompiledTree {
+  TreeProgram prog;
+  std::vector<TreeRoot> roots;
+  int n_outs = 0;
+  int n_regs = 0;             // registers the program uses
+  bool may_fail = false;      // contains an integer division or modulo: the error flag must be read back
+  std::vector<int> cols_read; // input columns the program loads, ascending
+};
+// Both fail with FLOCKGPU_ERR_UNSUPPORTED naming the limit when the program exceeds TREE_REGS registers,
+// TREE_MAX_INSTR instructions or TREE_POOL_BYTES of Utf8 literals, and for Boolean or computed Utf8 results.
+CompiledTree compile_tree_values(const std::vector<Expr>& exprs, const std::vector<ColInfo>& cols);
+CompiledTree compile_tree_predicate(const Expr& e, const std::vector<ColInfo>& cols);
+
+// ColInfo / ColRef views of a table's columns (filter_project.cu)
+std::vector<ColInfo> col_infos(const Table& t);
+void fill_colrefs(const Table& t, ColRef* refs);
 
 Expr tokens_to_expr(const flockgpu_expr* e);
 CompiledPredicate compile_predicate(const Expr& e, const std::vector<ColInfo>& cols);

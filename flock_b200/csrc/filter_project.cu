@@ -69,6 +69,37 @@ struct PredGenericT {
   }
 };
 
+// A predicate in the tree form (expr_tree.h): the verdict is the register program's result.  The register file sits in
+// the functor's shared staging area, two rows per thread at a time.
+template <int ROWS>
+struct PredTreeT {
+  static constexpr int E = 1;
+  static constexpr int I = ROWS;
+  static constexpr int MIN_CTAS = 1;
+  static constexpr bool ROUNDS = false;
+  static constexpr int R = 2;
+  struct Staged {  // thread t only touches slots [.][t]
+    Val v[TREE_REGS * R * FP_THREADS];
+    uint8_t f[TREE_REGS * R * FP_THREADS];
+  };
+  TreeProgram p;
+  __device__ __forceinline__ void load(Staged&, int64_t, int64_t, int) const {}
+  __device__ __forceinline__ unsigned long long test(const Staged& st, const ColRef* cols, int64_t tile_base, int64_t n_rows, int tid, int* err) const {
+    Staged& s = const_cast<Staged&>(st);  // the kernel's own shared variable
+    const TreeRegs<R, FP_THREADS> regs{s.v + tid, s.f + tid};
+    unsigned long long bits = 0;
+    for (int k = 0; k < I; k += R) {
+      int64_t rows[R];
+#pragma unroll
+      for (int j = 0; j < R; ++j) {
+        const int64_t r = tile_base + int64_t(k + j) * FP_THREADS + tid;
+        rows[j] = r < n_rows ? r : -1;
+      }
+      bits |= (unsigned long long)eval_tree<R>(p, cols, nullptr, rows, false, regs, err) << k;
+    }
+    return bits;
+  }
+};
 
 // other JOIN (group key, MIN / MAX) ON (k, v) against a direct-address group table (NEXMark q9: bids back to each
 // auction's top price): a row survives when k is inside the table's range, its slot is present and the slot's value
@@ -473,13 +504,13 @@ __global__ void __launch_bounds__(256) and_validity_kernel(const uint8_t* a, con
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-static std::vector<ColInfo> col_infos(const Table& t) {
+std::vector<ColInfo> col_infos(const Table& t) {
   std::vector<ColInfo> v;
   for (const Column& c : t.cols) v.push_back({c.dtype, c.name, c.format, c.validity != nullptr});
   return v;
 }
 
-static void fill_colrefs(const Table& t, ColRef* refs) {
+void fill_colrefs(const Table& t, ColRef* refs) {
   FG_CHECK(t.cols.size() <= size_t(MAX_IN_COLS), FLOCKGPU_ERR_UNSUPPORTED, "filter_project: more than %d input columns", MAX_IN_COLS);
   for (size_t i = 0; i < t.cols.size(); ++i) {
     FG_CHECK(!t.cols[i].all_null, FLOCKGPU_ERR_UNSUPPORTED, "filter_project: NULL input column \"%s\"", t.cols[i].name.c_str());
@@ -544,7 +575,12 @@ TablePtr filter_project(const CtxPtr& ctx, const TablePtr& in_ptr, const Expr* p
     std::vector<std::string> out_names;
     bool plain = true;
     for (size_t i = 0; i < projections.size() && plain; ++i) {
-      CompiledValue v = compile_value(projections[i], dinfos);
+      CompiledValue v;
+      try {
+        v = compile_value(projections[i], dinfos);
+      } catch (const Error& err) {
+        if (err.code != FLOCKGPU_ERR_UNSUPPORTED) throw;  // not a plain column: compiled again, for the tree form, below
+      }
       plain = v.passthrough;
       src.push_back(v.src_col);
       out_names.push_back(i < names.size() && !names[i].empty() ? names[i] : (plain ? in.cols[v.src_col].name : std::string()));
@@ -558,6 +594,7 @@ TablePtr filter_project(const CtxPtr& ctx, const TablePtr& in_ptr, const Expr* p
   std::vector<ColInfo> infos = col_infos(in);
   // ---- compile
   std::vector<CompiledValue> vals;
+  std::vector<bool> tree_vals;  // vals[i] is computed by the tree form
   if (projections.empty()) {
     for (size_t i = 0; i < in.cols.size(); ++i) {
       CompiledValue v;
@@ -568,8 +605,38 @@ TablePtr filter_project(const CtxPtr& ctx, const TablePtr& in_ptr, const Expr* p
       vals.push_back(v);
     }
   } else {
-    for (const Expr& e : projections) vals.push_back(compile_value(e, infos));
+    // an expression the chain form refuses is evaluated in the tree form (expr_eval.cu)
+    bool tree = false;
+    for (const Expr& e : projections) {
+      try {
+        CompiledValue v = compile_value(e, infos);
+        // the chain kernels read at most 4 validity inputs, and none inside the fused filter
+        int null_inputs = 0;
+        auto note = [&](int col) { null_inputs += col >= 0 && in.cols[col].validity; };
+        note(v.chain.start_col);
+        for (int st = 0; st < v.chain.n_steps; ++st)
+          if (v.chain.steps[st].src == 1) note(v.chain.steps[st].col);
+        if (!v.passthrough && null_inputs > (predicate ? 0 : 4)) fail(FLOCKGPU_ERR_UNSUPPORTED, "projection: more NULL inputs than the chain form carries");
+        vals.push_back(v);
+        tree_vals.push_back(false);
+      } catch (const Error& err) {
+        if (err.code != FLOCKGPU_ERR_UNSUPPORTED) throw;
+        const CompiledTree ct = compile_tree_values({e}, infos);  // fails when the tree form refuses it too
+        CompiledValue v;
+        v.dtype = ct.roots[0].dtype;
+        v.format = ct.roots[0].format;
+        vals.push_back(v);
+        tree_vals.push_back(true);
+        tree = true;
+      }
+    }
+    if (tree && predicate) {
+      // tree-form values are evaluated over the surviving rows only (a division by zero in a dropped row raises nothing)
+      TablePtr kept = filter_project(ctx, in_ptr, predicate, {}, {});
+      return filter_project(ctx, kept, nullptr, projections, names);
+    }
   }
+  tree_vals.resize(vals.size(), false);
   auto out_name = [&](size_t i) -> std::string {
     if (i < names.size() && !names[i].empty()) return names[i];
     if (vals[i].passthrough) return in.cols[vals[i].src_col].name;
@@ -611,7 +678,9 @@ TablePtr filter_project(const CtxPtr& ctx, const TablePtr& in_ptr, const Expr* p
       c.dtype = v.dtype;
       c.format = v.format;
       c.length = in.num_rows;
-      if (v.passthrough) {
+      if (tree_vals[i]) {
+        // filled in below: every tree-form column of the projection comes from one expr_eval_kernel launch
+      } else if (v.passthrough) {
         const Column& s = in.cols[v.src_col];
         c.nullable = s.nullable;
         c.data = s.data;  // zero-copy, like the Arc clone in ProjectionExec
@@ -668,6 +737,21 @@ TablePtr filter_project(const CtxPtr& ctx, const TablePtr& in_ptr, const Expr* p
       }
       out->cols.push_back(std::move(c));
     }
+    {
+      std::vector<Expr> tree_exprs;
+      std::vector<std::string> tree_names;
+      for (size_t i = 0; i < vals.size(); ++i)
+        if (tree_vals[i]) {
+          tree_exprs.push_back(projections[i]);
+          tree_names.push_back(out->cols[i].name);
+        }
+      if (!tree_exprs.empty()) {
+        std::vector<Column> computed = eval_exprs(ctx, in, tree_exprs, tree_names);
+        size_t k = 0;
+        for (size_t i = 0; i < vals.size(); ++i)
+          if (tree_vals[i]) out->cols[i] = std::move(computed[k++]);
+      }
+    }
     if (pa.n_out > 0 && in.num_rows > 0) {
       int64_t per_block = int64_t(PJ_THREADS) * PJ_ROWS;
       int grid = int(std::min<int64_t>((in.num_rows + per_block - 1) / per_block, int64_t(ctx->sm_count) * 8));
@@ -688,8 +772,19 @@ TablePtr filter_project(const CtxPtr& ctx, const TablePtr& in_ptr, const Expr* p
   }
 
   // -------------------------------------------------------------------- FilterExec (+ projection)
-  CompiledPredicate cp = compile_predicate(*predicate, infos);
-  check_err = cp.prog.has_div_by_col != 0;
+  CompiledPredicate cp;
+  CompiledTree tree_pred;  // the predicate in the tree form, when the term form refuses it
+  bool use_tree = false;
+  try {
+    cp = compile_predicate(*predicate, infos);
+  } catch (const Error& err) {
+    if (err.code != FLOCKGPU_ERR_UNSUPPORTED) throw;
+    tree_pred = compile_tree_predicate(*predicate, infos);
+    use_tree = true;
+    cp = CompiledPredicate{};
+    memset(&cp.prog, 0, sizeof cp.prog);
+  }
+  check_err = use_tree ? tree_pred.may_fail : cp.prog.has_div_by_col != 0;
   // host-resident (zero-copy) columns can be consumed in place only by the vectorised predicate with plain
   // pass-through fixed-width outputs; anything else scans the relation more than once and copies it to HBM first
   if (in.has_host_columns()) {
@@ -810,8 +905,15 @@ TablePtr filter_project(const CtxPtr& ctx, const TablePtr& in_ptr, const Expr* p
       launch_i32(0);
       break;
     default: {
-      if (in.num_rows >= int64_t(ctx->sm_count) * 4 * FP_THREADS * 16) launch(PredGenericT<16>{cp.prog});
-      else launch(PredGenericT<4>{cp.prog});
+      const bool large = in.num_rows >= int64_t(ctx->sm_count) * 4 * FP_THREADS * 16;
+      if (use_tree) {
+        if (large) launch(PredTreeT<16>{tree_pred.prog});
+        else launch(PredTreeT<4>{tree_pred.prog});
+      } else if (large) {
+        launch(PredGenericT<16>{cp.prog});
+      } else {
+        launch(PredGenericT<4>{cp.prog});
+      }
     }
   }
 

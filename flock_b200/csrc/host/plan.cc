@@ -95,8 +95,14 @@ static ExprTok scalar_token(const Json& value) {
   if (!value.is_object() || value.obj.size() != 1) fail(FLOCKGPU_ERR_INVALID, "plan JSON: malformed ScalarValue");
   const std::string& ty = value.obj[0].first;
   const Json& v = *value.obj[0].second;
-  if (v.is_null()) fail(FLOCKGPU_ERR_UNSUPPORTED, "plan: NULL literal of type %s", ty.c_str());
   ExprTok t{};
+  if (v.is_null()) {  // ScalarValue::Int64(None) and friends
+    t.op = FLOCKGPU_OP_LIT_NULL;
+    t.dtype = ty == "Float64" || ty == "Float32" ? FLOCKGPU_FLOAT64 : ty == "Utf8" || ty == "LargeUtf8" ? FLOCKGPU_UTF8 : ty == "Boolean" ? FLOCKGPU_BOOL
+              : ty == "Int32" ? FLOCKGPU_INT32 : ty == "UInt32" ? FLOCKGPU_UINT32 : ty == "UInt64" ? FLOCKGPU_UINT64
+              : ty.rfind("Timestamp", 0) == 0 ? FLOCKGPU_TIMESTAMP : FLOCKGPU_INT64;
+    return t;
+  }
   if (ty == "Float64" || ty == "Float32") {
     t.op = FLOCKGPU_OP_LIT_F64;
     t.dtype = FLOCKGPU_FLOAT64;
@@ -154,9 +160,98 @@ static void emit_expr(const Json& e, const fg::Table& in, Expr* out) {
     ExprTok t{};
     t.op = FLOCKGPU_OP_NOT;
     out->push_back(t);
+  } else if (kind == "negative_expr" || kind == "negative" || kind == "is_null_expr" || kind == "is_null" || kind == "is_not_null_expr" ||
+             kind == "is_not_null") {
+    emit_expr(e.get("arg") ? e.at("arg") : e.at("expr"), in, out);
+    ExprTok t{};
+    t.op = kind[0] == 'n' ? FLOCKGPU_OP_NEG : kind.rfind("is_not", 0) == 0 ? FLOCKGPU_OP_IS_NOT_NULL : FLOCKGPU_OP_IS_NULL;
+    out->push_back(t);
+  } else if (kind == "case_expr" || kind == "case") {
+    // DataFusion 6 CaseExpr { expr: Option, when_then_expr: Vec<(when, then)>, else_expr: Option }
+    ExprTok t{};
+    t.op = FLOCKGPU_OP_CASE;
+    const Json* base = e.get("expr");
+    if (base && !base->is_null()) {
+      emit_expr(*base, in, out);
+      t.col |= FLOCKGPU_CASE_HAS_BASE;
+    }
+    const Json& wt = e.at("when_then_expr");
+    if (!wt.is_array() || wt.arr.empty()) fail(FLOCKGPU_ERR_INVALID, "plan JSON: case_expr without when_then_expr pairs");
+    for (const JsonPtr& pair : wt.arr) {
+      if (!pair->is_array() || pair->arr.size() != 2) fail(FLOCKGPU_ERR_INVALID, "plan JSON: when_then_expr entries must be [when, then]");
+      emit_expr(*pair->arr[0], in, out);
+      emit_expr(*pair->arr[1], in, out);
+    }
+    t.i64 = int64_t(wt.arr.size());
+    const Json* els = e.get("else_expr");
+    if (els && !els->is_null()) {
+      emit_expr(*els, in, out);
+      t.col |= FLOCKGPU_CASE_HAS_ELSE;
+    }
+    out->push_back(t);
+  } else if (kind == "in_list_expr" || kind == "in_list") {
+    // InListExpr { expr, list, negated }
+    emit_expr(e.at("expr"), in, out);
+    const Json& list = e.at("list");
+    if (!list.is_array() || list.arr.empty()) fail(FLOCKGPU_ERR_INVALID, "plan JSON: in_list_expr without a list");
+    for (const JsonPtr& l : list.arr) emit_expr(*l, in, out);
+    ExprTok t{};
+    t.op = FLOCKGPU_OP_IN_LIST;
+    t.i64 = int64_t(list.arr.size());
+    const Json* neg = e.get("negated");
+    t.col = neg && neg->kind == Json::Bool && neg->b ? 1 : 0;
+    out->push_back(t);
   } else {
     fail(FLOCKGPU_ERR_UNSUPPORTED, "plan: physical expression \"%s\" is not supported on the GPU path", kind.c_str());
   }
+}
+
+// The input columns that hold the values of `exprs` (a null entry gives -1): a plain column is itself; all the others
+// are evaluated by ONE expr_eval_kernel launch into hidden columns appended to *in.
+static std::vector<int> expr_columns(const ExecEnv& env, TablePtr* in, const std::vector<const Json*>& exprs) {
+  std::vector<int> cols(exprs.size(), -1);
+  std::vector<Expr> computed;
+  std::vector<std::string> names;
+  std::vector<size_t> where;
+  for (size_t i = 0; i < exprs.size(); ++i) {
+    if (!exprs[i]) continue;
+    if (is_column_expr(*exprs[i])) {
+      cols[i] = column_of(*exprs[i], **in);
+      continue;
+    }
+    Expr t;
+    emit_expr(*exprs[i], **in, &t);
+    computed.push_back(std::move(t));
+    names.push_back("__expr" + std::to_string(i));
+    where.push_back(i);
+  }
+  if (computed.empty()) return cols;
+  (*in)->dense();
+  std::vector<fg::Column> vals = fg::eval_exprs(env.ctx, **in, computed, names);
+  auto wide = std::make_shared<fg::Table>(**in);
+  for (size_t k = 0; k < vals.size(); ++k) {
+    cols[where[k]] = int(wide->cols.size());
+    wide->cols.push_back(std::move(vals[k]));
+  }
+  *in = wide;
+  return cols;
+}
+
+// Group columns and aggregate arguments of a Partial / Single aggregate over *in (COUNT over a literal is COUNT(*): -1).
+static void aggregate_columns(const ExecEnv& env, const HashAggregateExec& n, TablePtr* in, std::vector<int>* gcols, std::vector<int>* acols) {
+  std::vector<const Json*> exprs;
+  for (const auto& g : n.group_expr) exprs.push_back(g.first);
+  for (const auto& a : n.aggr_expr) {
+    const Json* k = a.expr ? a.expr->get("physical_expr") : nullptr;
+    const bool literal = k && k->is_string() && k->str == "literal";
+    exprs.push_back(a.func == FLOCKGPU_AGG_COUNT && literal ? nullptr : a.expr);
+  }
+  const std::vector<int> cols = expr_columns(env, in, exprs);
+  gcols->assign(cols.begin(), cols.begin() + n.group_expr.size());
+  acols->assign(cols.begin() + n.group_expr.size(), cols.end());
+  for (size_t i = 0; i < acols->size(); ++i)
+    if (n.aggr_expr[i].func != FLOCKGPU_AGG_COUNT && (*acols)[i] < 0)
+      fail(FLOCKGPU_ERR_UNSUPPORTED, "HashAggregateExec: aggregate \"%s\" has no argument", n.aggr_expr[i].name.c_str());
 }
 
 static std::string data_type_display(const Json& j) {
@@ -198,6 +293,28 @@ static std::string expr_display(const Json& e) {
     for (const auto& kv : sym)
       if (op == kv.first) op = kv.second;
     return expr_display(e.at("left")) + " " + op + " " + expr_display(e.at("right"));
+  }
+  if (kind == "not_expr" || kind == "not") return "NOT " + expr_display(e.get("arg") ? e.at("arg") : e.at("expr"));
+  if (kind == "negative_expr" || kind == "negative") return "(- " + expr_display(e.get("arg") ? e.at("arg") : e.at("expr")) + ")";
+  if (kind == "is_null_expr" || kind == "is_null") return expr_display(e.get("arg") ? e.at("arg") : e.at("expr")) + " IS NULL";
+  if (kind == "is_not_null_expr" || kind == "is_not_null") return expr_display(e.get("arg") ? e.at("arg") : e.at("expr")) + " IS NOT NULL";
+  if (kind == "case_expr" || kind == "case") {
+    std::string s = "CASE ";
+    const Json* base = e.get("expr");
+    if (base && !base->is_null()) s += expr_display(*base) + " ";
+    if (const Json* wt = e.get("when_then_expr"))
+      for (const JsonPtr& pair : wt->arr)
+        if (pair->is_array() && pair->arr.size() == 2) s += "WHEN " + expr_display(*pair->arr[0]) + " THEN " + expr_display(*pair->arr[1]) + " ";
+    const Json* els = e.get("else_expr");
+    if (els && !els->is_null()) s += "ELSE " + expr_display(*els) + " ";
+    return s + "END";
+  }
+  if (kind == "in_list_expr" || kind == "in_list") {
+    const Json* neg = e.get("negated");
+    std::string s = expr_display(e.at("expr")) + (neg && neg->kind == Json::Bool && neg->b ? " NOT IN ([" : " IN ([");
+    if (const Json* list = e.get("list"))
+      for (size_t i = 0; i < list->arr.size(); ++i) s += (i ? ", " : "") + expr_display(*list->arr[i]);
+    return s + "])";
   }
   return kind;
 }
@@ -516,14 +633,10 @@ TablePtr HashAggregateExec::execute_uncached(const ExecEnv& env) {
         JoinCount jc = join_count(env, *partial, count_names);
         if (jc.counted) return rename_columns(env, jc.counted, group_names);
         TablePtr in = jc.joined ? jc.joined : partial->input->execute(env);
-        std::vector<int> gcols = group_columns(*partial, *in);
+        std::vector<int> gcols, acols;
+        aggregate_columns(env, *partial, &in, &gcols, &acols);
         std::vector<fg::AggSpec> specs;
-        for (size_t i = 0; i < partial->aggr_expr.size(); ++i) {
-          const auto& a = partial->aggr_expr[i];
-          int col = a.expr && is_column_expr(*a.expr) ? column_of(*a.expr, *in) : -1;
-          if (a.func != FLOCKGPU_AGG_COUNT && col < 0) fail(FLOCKGPU_ERR_UNSUPPORTED, "HashAggregateExec: aggregate argument must be a plain column");
-          specs.push_back(fg::AggSpec{a.func, col, aggr_expr[i].name});
-        }
+        for (size_t i = 0; i < partial->aggr_expr.size(); ++i) specs.push_back(fg::AggSpec{partial->aggr_expr[i].func, acols[i], aggr_expr[i].name});
         TablePtr out = fg::hash_aggregate(env.ctx, in, FLOCKGPU_AGG_SINGLE, gcols, specs);
         std::vector<std::string> names;
         for (const auto& g : group_expr) names.push_back(g.second);
@@ -540,7 +653,9 @@ TablePtr HashAggregateExec::execute_uncached(const ExecEnv& env) {
     if (jc.counted) return rename_columns(env, jc.counted, group_names);
   }
   TablePtr in = jc.joined ? jc.joined : input->execute(env);
-  std::vector<int> gcols = group_columns(*this, *in);
+  std::vector<int> gcols, acols;
+  if (final_mode) gcols = group_columns(*this, *in);  // a Final aggregate reads its group and state columns by position
+  else aggregate_columns(env, *this, &in, &gcols, &acols);
   // A Partial DISTINCT (no aggregate functions) ahead of a shuffle only exists to shrink what travels.  With Utf8 / wide
   // group keys it costs a full row-representative hash table (q8: 2.5 M persons that are all different), so
   // ask a sample first: when (nearly) every key of the first 64 Ki rows is new, the rows themselves are the partial
@@ -569,11 +684,7 @@ TablePtr HashAggregateExec::execute_uncached(const ExecEnv& env) {
   }
   std::vector<fg::AggSpec> specs;
   if (!final_mode) {
-    for (const auto& a : aggr_expr) {
-      int col = a.expr && is_column_expr(*a.expr) ? column_of(*a.expr, *in) : -1;
-      if (a.func != FLOCKGPU_AGG_COUNT && col < 0) fail(FLOCKGPU_ERR_UNSUPPORTED, "HashAggregateExec: aggregate argument must be a plain column");
-      specs.push_back(fg::AggSpec{a.func, col, a.name});
-    }
+    for (size_t i = 0; i < aggr_expr.size(); ++i) specs.push_back(fg::AggSpec{aggr_expr[i].func, acols[i], aggr_expr[i].name});
   } else {
     // the partial output is [group columns..., state columns in aggregate order]
     int state = int(group_expr.size());
@@ -617,12 +728,18 @@ std::string SortExec::fmt_as() const {
 TablePtr SortExec::execute(const ExecEnv& env) {
   TablePtr in = input->execute(env);
   in->resolve();
+  const size_t n_cols = in->cols.size();
+  std::vector<const Json*> exprs;
+  for (const Key& k : expr) exprs.push_back(k.expr);
+  const std::vector<int> cols = expr_columns(env, &in, exprs);
   std::vector<fg::SortKey> keys;
-  for (const Key& k : expr) {
-    if (!is_column_expr(*k.expr)) fail(FLOCKGPU_ERR_UNSUPPORTED, "SortExec: sort expressions must be plain columns on the GPU path");
-    keys.push_back(fg::SortKey{column_of(*k.expr, *in), k.descending, k.nulls_first});
-  }
-  return fg::sort_table(env.ctx, in, keys);
+  for (size_t i = 0; i < expr.size(); ++i) keys.push_back(fg::SortKey{cols[i], expr[i].descending, expr[i].nulls_first});
+  TablePtr sorted = fg::sort_table(env.ctx, in, keys);
+  if (sorted->cols.size() == n_cols) return sorted;
+  sorted->resolve();
+  auto out = std::make_shared<fg::Table>(*sorted);  // without the computed keys
+  out->cols.resize(n_cols);
+  return out;
 }
 
 TablePtr GlobalLimitExec::execute(const ExecEnv& env) { return fg::limit_rows(env.ctx, input->execute(env), limit); }

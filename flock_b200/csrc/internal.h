@@ -497,6 +497,10 @@ TablePtr empty_like(const CtxPtr& ctx, const Table& t);
 TablePtr filter_project(const CtxPtr& ctx, const TablePtr& in, const Expr* predicate,
                         const std::vector<Expr>& projections, const std::vector<std::string>& names);
 
+// The values of `exprs` over `in`, one column each (named names[i], or derived), with ONE expr_eval_kernel launch for
+// all of them (expr_eval.cu); plain columns share the input's buffers.  Runs the tree form (expr_tree.h).
+std::vector<Column> eval_exprs(const CtxPtr& ctx, const Table& in, const std::vector<Expr>& exprs, const std::vector<std::string>& names);
+
 struct AggSpec {
   int func;
   int col;

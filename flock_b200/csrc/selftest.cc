@@ -103,6 +103,43 @@ int flockgpu_selftest_eval_value(const struct ArrowSchema* schema, const struct 
   });
 }
 
+// The tree form: all of `exprs` as ONE register program (or exprs[0] as a predicate), run by eval_tree compiled for the
+// host with a private register file.
+int flockgpu_selftest_eval_tree(const struct ArrowSchema* schema, const struct ArrowArray* batch, const flockgpu_expr* exprs, int32_t n_exprs,
+                                int32_t predicate, void* const* out_values, uint8_t* const* out_valid, int32_t* out_dtypes,
+                                int32_t* out_passthrough, int32_t* out_n_instr) {
+  return guarded([&] {
+    FG_CHECK(exprs && n_exprs >= 1 && out_values && (!predicate || n_exprs == 1), FLOCKGPU_ERR_INVALID, "selftest_eval_tree: bad arguments");
+    HostBatch hb = view_batch(schema, batch);
+    std::vector<Expr> es;
+    for (int i = 0; i < n_exprs; ++i) es.push_back(tokens_to_expr(&exprs[i]));
+    const CompiledTree ct = predicate ? compile_tree_predicate(es[0], hb.infos) : compile_tree_values(es, hb.infos);
+    if (out_n_instr) *out_n_instr = ct.prog.n_instr;
+    std::vector<TreeOut> outs(TREE_MAX_OUTS);
+    if (!predicate) {
+      FG_CHECK(out_valid && out_dtypes && out_passthrough, FLOCKGPU_ERR_INVALID, "selftest_eval_tree: bad arguments");
+      for (int i = 0; i < n_exprs; ++i) {
+        const TreeRoot& r = ct.roots[size_t(i)];
+        out_dtypes[i] = r.dtype;
+        out_passthrough[i] = r.passthrough ? 1 : 0;
+        if (r.passthrough) continue;
+        memset(out_valid[i], 1, size_t(hb.rows));
+        outs[size_t(r.out)] = TreeOut{out_values[i], r.may_be_null ? out_valid[i] : nullptr, r.dtype, 0};
+      }
+    }
+    Val reg_val[TREE_REGS];
+    uint8_t reg_flag[TREE_REGS];
+    const TreeRegs<1, 1> regs{reg_val, reg_flag};
+    int err = 0;
+    for (int64_t r = 0; r < hb.rows; ++r) {
+      int64_t rows[1] = {r};
+      const unsigned keep = eval_tree<1>(ct.prog, hb.refs.data(), outs.data(), rows, false, regs, &err);
+      if (predicate) static_cast<uint8_t*>(out_values[0])[r] = uint8_t(keep & 1u);
+    }
+    FG_CHECK(!err, FLOCKGPU_ERR_EXECUTION, "Divide by zero");
+  });
+}
+
 }  // extern "C"
 
 // The vectorised predicate `CAST(x AS Int64) [% modulus] cmp rhs` (modulus = 0: no `%`) exactly as the filter kernel

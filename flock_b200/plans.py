@@ -59,6 +59,30 @@ def try_cast(expr: dict, type_json) -> dict:
     return {"physical_expr": "try_cast_expr", "expr": expr, "cast_type": type_json}
 
 
+# The reference's fixtures serialise no CASE, IN list, IS NULL or unary minus: the tags below follow the snake-cased
+# struct names like the tags the fixtures do show (binary_expr, try_cast_expr), with DataFusion 6's field names.
+def case_expr(when_then: list[tuple[dict, dict]], else_expr: dict | None = None, expr: dict | None = None) -> dict:
+    """CaseExpr { expr, when_then_expr, else_expr }: CASE [expr] WHEN w THEN t ... [ELSE else_expr] END."""
+    return {"physical_expr": "case_expr", "expr": expr, "when_then_expr": [[w, t] for w, t in when_then], "else_expr": else_expr}
+
+
+def in_list(expr: dict, values: list[dict], negated: bool = False) -> dict:
+    """InListExpr { expr, list, negated }."""
+    return {"physical_expr": "in_list_expr", "expr": expr, "list": values, "negated": negated}
+
+
+def is_null(arg: dict) -> dict:
+    return {"physical_expr": "is_null_expr", "arg": arg}
+
+
+def is_not_null(arg: dict) -> dict:
+    return {"physical_expr": "is_not_null_expr", "arg": arg}
+
+
+def negative(arg: dict) -> dict:
+    return {"physical_expr": "negative_expr", "arg": arg}
+
+
 # ---- execution plans -------------------------------------------------------------------------------------
 def memory_exec(schema: pa.Schema, projection: list[int] | None) -> dict:
     return {"execution_plan": "memory_exec", "schema": schema_json(schema), "projection": projection}

@@ -260,8 +260,24 @@ enum flockgpu_op {
   FLOCKGPU_OP_MOD = 14,     /* truncated remainder, sign of the dividend (Rust `%`)              */
   FLOCKGPU_OP_EQ = 20, FLOCKGPU_OP_NE = 21, FLOCKGPU_OP_LT = 22, FLOCKGPU_OP_LE = 23,
   FLOCKGPU_OP_GT = 24, FLOCKGPU_OP_GE = 25,
-  FLOCKGPU_OP_AND = 30, FLOCKGPU_OP_OR = 31, FLOCKGPU_OP_NOT = 32
+  FLOCKGPU_OP_AND = 30, FLOCKGPU_OP_OR = 31, FLOCKGPU_OP_NOT = 32,
+  /* Expression trees (negative_expr, is_null_expr, is_not_null_expr, NULL ScalarValues, case_expr, in_list_expr).
+   * AND / OR / NOT results may also be used as values (inside CASE, under IS NULL, ...).                      */
+  FLOCKGPU_OP_NEG = 40,         /* pop x, push -x (signed integers wrap, Float64 flips the sign)            */
+  FLOCKGPU_OP_IS_NULL = 41,     /* pop x, push x IS NULL (never NULL itself)                                */
+  FLOCKGPU_OP_IS_NOT_NULL = 42, /* pop x, push x IS NOT NULL                                                */
+  FLOCKGPU_OP_LIT_NULL = 43,    /* push a NULL literal of type `dtype`                                      */
+  /* CASE [base] WHEN w1 THEN t1 ... WHEN wn THEN tn [ELSE e] END: i64 = n (>= 1), col bit 0 = "has base", bit 1 =
+   * "has else"; pops, in push order, [base] w1 t1 ... wn tn [e].  Without a base every w is boolean; with one the
+   * branch is taken when base = w.  A condition that is FALSE or NULL falls through; no ELSE gives NULL.           */
+  FLOCKGPU_OP_CASE = 44,
+  /* x [NOT] IN (l1 ... ln): i64 = n (>= 1), col = 1 for NOT IN; pops, in push order, x l1 ... ln, where every l is a
+   * literal token (LIT_I64 / LIT_F64 / LIT_UTF8 / LIT_NULL).  SQL's three-valued result: NULL when x is NULL, or when
+   * nothing matches and a list literal is NULL.                                                                      */
+  FLOCKGPU_OP_IN_LIST = 45
 };
+#define FLOCKGPU_CASE_HAS_BASE 1
+#define FLOCKGPU_CASE_HAS_ELSE 2
 typedef struct flockgpu_expr_token {
   int32_t op;      /* enum flockgpu_op                                      */
   int32_t dtype;   /* enum flockgpu_dtype: CAST target / literal type       */
@@ -406,6 +422,16 @@ int flockgpu_selftest_eval_predicate(const struct ArrowSchema* schema, const str
 int flockgpu_selftest_eval_value(const struct ArrowSchema* schema, const struct ArrowArray* batch,
                                  const flockgpu_expr* expr, void* out, int32_t* out_dtype,
                                  int32_t* out_passthrough);
+/* CPU-only: the TREE form (flock_b200/csrc/expr_tree.h), which the operators use for what the term/chain forms refuse:
+ * compiles `n_exprs` value expressions into ONE register program (or, with `predicate` != 0, exprs[0] as a filter
+ * predicate) and runs it over a host record batch with the kernels' interpreter compiled for the host.
+ * Values: out_values[k] holds rows * 8 bytes (4-byte types packed), out_valid[k] rows bytes (1 = not NULL),
+ * out_dtypes[k] the result type, out_passthrough[k] = 1 for a plain column (nothing written).  Predicate:
+ * out_values[0] receives rows bytes, 1 = the row is kept (the predicate is TRUE).  *out_n_instr (may be NULL) = number of
+ * instructions of the program.                                                                                    */
+int flockgpu_selftest_eval_tree(const struct ArrowSchema* schema, const struct ArrowArray* batch, const flockgpu_expr* exprs,
+                                int32_t n_exprs, int32_t predicate, void* const* out_values, uint8_t* const* out_valid,
+                                int32_t* out_dtypes, int32_t* out_passthrough, int32_t* out_n_instr);
 /* CPU-only: the arithmetic of the vectorised filter predicate CAST(x AS Int64) [% modulus] cmp rhs (modulus 0 = no `%`),
  * with the constants and the per-row test the GPU kernel uses (flock_b200/csrc/pred_i32.h).  out_keep[i] in {0, 1}. */
 int flockgpu_selftest_pred_i32(int64_t modulus, int32_t cmp, int64_t rhs, const int32_t* x, int64_t n, uint8_t* out_keep, int32_t* out_mode);
