@@ -24,16 +24,18 @@ from ._ffi import FlockGpuError, lib, check
 __all__ = ["Context", "Table", "HostRelation", "ExecutionContext", "Window", "FlockGpuError", "col", "lit", "null", "case", "E"]
 
 # enum flockgpu_dtype
-BOOL, INT32, INT64, UINT64, FLOAT64, TIMESTAMP, UTF8, UINT32 = range(8)
+BOOL, INT32, INT64, UINT64, FLOAT64, TIMESTAMP, UTF8, UINT32, DATE32 = range(9)
 _DTYPE_BY_NAME = {"bool": BOOL, "int32": INT32, "int64": INT64, "uint64": UINT64, "float64": FLOAT64,
-                  "timestamp": TIMESTAMP, "utf8": UTF8, "uint32": UINT32,
-                  "Int32": INT32, "Int64": INT64, "UInt64": UINT64, "Float64": FLOAT64, "Utf8": UTF8, "UInt32": UINT32}
+                  "timestamp": TIMESTAMP, "utf8": UTF8, "uint32": UINT32, "date32": DATE32,
+                  "Int32": INT32, "Int64": INT64, "UInt64": UINT64, "Float64": FLOAT64, "Utf8": UTF8, "UInt32": UINT32,
+                  "Date32": DATE32}
 # enum flockgpu_op
 OP_COLUMN, OP_LIT_I64, OP_LIT_F64, OP_LIT_UTF8, OP_CAST = 1, 2, 3, 4, 5
 OP_ADD, OP_SUB, OP_MUL, OP_DIV, OP_MOD = 10, 11, 12, 13, 14
 OP_EQ, OP_NE, OP_LT, OP_LE, OP_GT, OP_GE = 20, 21, 22, 23, 24, 25
 OP_AND, OP_OR, OP_NOT = 30, 31, 32
 OP_NEG, OP_IS_NULL, OP_IS_NOT_NULL, OP_LIT_NULL, OP_CASE, OP_IN_LIST = 40, 41, 42, 43, 44, 45
+OP_LIKE, OP_NOT_LIKE = 46, 47
 CASE_HAS_BASE, CASE_HAS_ELSE = 1, 2
 # enum flockgpu_agg_mode / flockgpu_agg_func
 AGG_PARTIAL, AGG_FINAL, AGG_FINAL_PARTITIONED, AGG_SINGLE = 0, 1, 2, 3
@@ -89,6 +91,10 @@ class E:
     def __neg__(self): return E(self.tokens + [(OP_NEG, 0, 0, 0, 0.0, None)])
     def is_null(self) -> "E": return E(self.tokens + [(OP_IS_NULL, 0, 0, 0, 0.0, None)])
     def is_not_null(self) -> "E": return E(self.tokens + [(OP_IS_NOT_NULL, 0, 0, 0, 0.0, None)])
+
+    def like(self, pattern, negated: bool = False) -> "E":
+        """self [NOT] LIKE pattern (a str, or None for a NULL pattern)."""
+        return self._bin(OP_NOT_LIKE if negated else OP_LIKE, null("utf8") if pattern is None else pattern)
 
     def isin(self, values, negated: bool = False) -> "E":
         """self [NOT] IN (values): literals (None = a NULL literal)."""
@@ -599,7 +605,7 @@ def selftest_eval_tree(batch: pa.RecordBatch, exprs, predicate: bool = False):
         _release_exported(c_schema, arrays, 1)
     if predicate:
         return vals[0].view(np.uint8)[:n].astype(bool), n_instr.value
-    views = {INT32: np.int32, UINT32: np.uint32, FLOAT64: np.float64, UINT64: np.uint64}
+    views = {INT32: np.int32, UINT32: np.uint32, DATE32: np.int32, FLOAT64: np.float64, UINT64: np.uint64}
     out = []
     for i in range(k):
         v = None if passes[i] else vals[i].view(views.get(dts[i], np.int64))[:n].copy()

@@ -41,7 +41,7 @@ void fail(int code, const char* fmt, ...) {
 int dtype_width(int dtype) {
   switch (dtype) {
     case FLOCKGPU_BOOL: return 1;
-    case FLOCKGPU_INT32: case FLOCKGPU_UINT32: return 4;
+    case FLOCKGPU_INT32: case FLOCKGPU_UINT32: case FLOCKGPU_DATE32: return 4;
     case FLOCKGPU_INT64: case FLOCKGPU_UINT64: case FLOCKGPU_FLOAT64: case FLOCKGPU_TIMESTAMP: return 8;
     default: return 0;
   }
@@ -56,6 +56,7 @@ const char* dtype_name(int dtype) {
     case FLOCKGPU_UINT64: return "UInt64";
     case FLOCKGPU_FLOAT64: return "Float64";
     case FLOCKGPU_TIMESTAMP: return "Timestamp";
+    case FLOCKGPU_DATE32: return "Date32";
     case FLOCKGPU_UTF8: return "Utf8";
     default: return "?";
   }
@@ -69,6 +70,7 @@ int dtype_from_format(const char* f) {
   if (!strcmp(f, "L")) return FLOCKGPU_UINT64;
   if (!strcmp(f, "g")) return FLOCKGPU_FLOAT64;
   if (!strcmp(f, "u")) return FLOCKGPU_UTF8;
+  if (!strcmp(f, "tdD")) return FLOCKGPU_DATE32;
   if (!strncmp(f, "ts", 2) && strlen(f) >= 4 && f[3] == ':') return FLOCKGPU_TIMESTAMP;
   return -1;
 }
@@ -82,6 +84,7 @@ std::string default_format(int dtype) {
     case FLOCKGPU_FLOAT64: return "g";
     case FLOCKGPU_UTF8: return "u";
     case FLOCKGPU_TIMESTAMP: return "tsm:";
+    case FLOCKGPU_DATE32: return "tdD";
     default: return "n";
   }
 }

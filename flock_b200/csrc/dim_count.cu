@@ -139,7 +139,7 @@ static ColRef colref_of(const Column& c) {
 }
 
 bool dim_count_key_type(int dtype) {
-  return dtype == FLOCKGPU_INT32 || dtype == FLOCKGPU_INT64 || dtype == FLOCKGPU_UINT64 || dtype == FLOCKGPU_TIMESTAMP || dtype == FLOCKGPU_UTF8;
+  return dtype == FLOCKGPU_INT32 || dtype == FLOCKGPU_DATE32 || dtype == FLOCKGPU_INT64 || dtype == FLOCKGPU_UINT64 || dtype == FLOCKGPU_TIMESTAMP || dtype == FLOCKGPU_UTF8;
 }
 
 TablePtr dim_count_aggregate(const CtxPtr& ctx, const TablePtr& fact_ptr, int fact_key, const Expr* predicate, const TablePtr& dim_ptr, int dim_key,

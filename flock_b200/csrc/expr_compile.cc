@@ -39,6 +39,9 @@ bool is_intlike(int dt) {
 }
 bool is_unsigned(int dt) { return dt == FLOCKGPU_UINT32 || dt == FLOCKGPU_UINT64; }
 bool is_numeric(int dt) { return is_intlike(dt) || dt == FLOCKGPU_FLOAT64; }
+// Date32 is neither: it compares with Date32 only and takes part in no arithmetic or cast, and is lowered as Int32 is
+bool same_ordered(int a, int b) { return a == b && (a == FLOCKGPU_UTF8 || a == FLOCKGPU_DATE32); }
+bool is_i32(int dt) { return dt == FLOCKGPU_INT32 || dt == FLOCKGPU_DATE32; }
 
 int promote(int a, int b) {
   if (a == b) return a;
@@ -81,7 +84,7 @@ Tree build_tree(const Expr& e, const std::vector<ColInfo>& cols) {
       case FLOCKGPU_OP_LIT_I64:
         n.i = tok.i64;
         n.dtype = (tok.dtype == FLOCKGPU_INT32 || tok.dtype == FLOCKGPU_UINT32 || tok.dtype == FLOCKGPU_UINT64 ||
-                   tok.dtype == FLOCKGPU_TIMESTAMP)
+                   tok.dtype == FLOCKGPU_TIMESTAMP || tok.dtype == FLOCKGPU_DATE32)
                       ? tok.dtype
                       : FLOCKGPU_INT64;
         break;
@@ -105,7 +108,7 @@ Tree build_tree(const Expr& e, const std::vector<ColInfo>& cols) {
         FG_CHECK(t.nodes[n.l].dtype == FLOCKGPU_BOOL, FLOCKGPU_ERR_INVALID, "expression: NOT of a non-boolean");
         break;
       case FLOCKGPU_OP_LIT_NULL:
-        FG_CHECK(tok.dtype >= FLOCKGPU_BOOL && tok.dtype <= FLOCKGPU_UINT32, FLOCKGPU_ERR_INVALID, "expression: NULL literal of unknown type %d", tok.dtype);
+        FG_CHECK(tok.dtype >= FLOCKGPU_BOOL && tok.dtype <= FLOCKGPU_DATE32, FLOCKGPU_ERR_INVALID, "expression: NULL literal of unknown type %d", tok.dtype);
         n.dtype = tok.dtype;
         break;
       case FLOCKGPU_OP_NEG:
@@ -136,7 +139,7 @@ Tree build_tree(const Expr& e, const std::vector<ColInfo>& cols) {
           if (!is_value) {
             if (has_base) {
               const int bt = t.nodes[n.kids[0]].dtype;
-              FG_CHECK((is_numeric(bt) && is_numeric(c.dtype)) || (bt == FLOCKGPU_UTF8 && c.dtype == FLOCKGPU_UTF8), FLOCKGPU_ERR_UNSUPPORTED,
+              FG_CHECK((is_numeric(bt) && is_numeric(c.dtype)) || same_ordered(bt, c.dtype), FLOCKGPU_ERR_UNSUPPORTED,
                        "expression: CASE compares %s with %s", dtype_name(bt), dtype_name(c.dtype));
             } else {
               FG_CHECK(c.dtype == FLOCKGPU_BOOL, FLOCKGPU_ERR_INVALID, "expression: CASE WHEN condition is not boolean");
@@ -165,9 +168,20 @@ Tree build_tree(const Expr& e, const std::vector<ColInfo>& cols) {
         for (size_t k = 1; k < n.kids.size(); ++k) {
           const Node& c = t.nodes[n.kids[k]];
           FG_CHECK(is_literal(c) || c.op == FLOCKGPU_OP_LIT_NULL, FLOCKGPU_ERR_INVALID, "expression: IN list entry %zu is not a literal", k - 1);
-          FG_CHECK(c.op == FLOCKGPU_OP_LIT_NULL || (is_numeric(vt) && is_numeric(c.dtype)) || (vt == FLOCKGPU_UTF8 && c.dtype == FLOCKGPU_UTF8),
+          FG_CHECK(c.op == FLOCKGPU_OP_LIT_NULL || (is_numeric(vt) && is_numeric(c.dtype)) || same_ordered(vt, c.dtype),
                    FLOCKGPU_ERR_UNSUPPORTED, "expression: %s IN a list with a %s literal", dtype_name(vt), dtype_name(c.dtype));
         }
+        n.dtype = FLOCKGPU_BOOL;
+        break;
+      }
+      case FLOCKGPU_OP_LIKE:
+      case FLOCKGPU_OP_NOT_LIKE: {
+        n.r = pop();
+        n.l = pop();
+        const Node& v = t.nodes[n.l];
+        const Node& pat = t.nodes[n.r];
+        FG_CHECK(v.dtype == FLOCKGPU_UTF8 || v.op == FLOCKGPU_OP_LIT_NULL, FLOCKGPU_ERR_UNSUPPORTED, "expression: LIKE over %s", dtype_name(v.dtype));
+        FG_CHECK(pat.op == FLOCKGPU_OP_LIT_UTF8 || pat.op == FLOCKGPU_OP_LIT_NULL, FLOCKGPU_ERR_UNSUPPORTED, "expression: LIKE needs a literal pattern");
         n.dtype = FLOCKGPU_BOOL;
         break;
       }
@@ -181,7 +195,7 @@ Tree build_tree(const Expr& e, const std::vector<ColInfo>& cols) {
                      dtype_name(rt));
             n.dtype = promote(lt, rt);
           } else if (is_cmp(tok.op)) {
-            FG_CHECK((is_numeric(lt) && is_numeric(rt)) || (lt == FLOCKGPU_UTF8 && rt == FLOCKGPU_UTF8), FLOCKGPU_ERR_UNSUPPORTED,
+            FG_CHECK((is_numeric(lt) && is_numeric(rt)) || same_ordered(lt, rt), FLOCKGPU_ERR_UNSUPPORTED,
                      "expression: comparison of %s with %s", dtype_name(lt), dtype_name(rt));
             n.dtype = FLOCKGPU_BOOL;
           } else {
@@ -208,7 +222,7 @@ Val literal_as(const Node& n, int dtype) {
     v.d = n.op == FLOCKGPU_OP_LIT_F64 ? n.d : (is_unsigned(n.dtype) ? double(uint64_t(n.i)) : double(n.i));
   } else {
     int64_t x = n.op == FLOCKGPU_OP_LIT_F64 ? int64_t(n.d) : n.i;
-    if (dtype == FLOCKGPU_INT32) x = int64_t(int32_t(uint32_t(uint64_t(x))));
+    if (is_i32(dtype)) x = int64_t(int32_t(uint32_t(uint64_t(x))));
     if (dtype == FLOCKGPU_UINT32) x = int64_t(uint64_t(uint32_t(uint64_t(x))));
     v.i = x;
   }
@@ -571,7 +585,7 @@ CompiledPredicate compile_predicate(const Expr& e, const std::vector<ColInfo>& c
     return out;  // no vectorised shape reads validity
   }
 
-  // fast shapes: one term over one Int32 column against literals
+  // fast shapes: one term over one Int32 (or Date32) column against literals
   // (a single term has a 2-entry truth table: 0b10 = the term itself, 0b01 = NOT term; constants keep the interpreter)
   const unsigned table1 = p.lut[0] & 3u;
   auto negate_cmp = [](int cmp) {
@@ -588,7 +602,7 @@ CompiledPredicate compile_predicate(const Expr& e, const std::vector<ColInfo>& c
     const Term& term = p.terms[0];
     const Chain& l = term.lhs;
     const Chain& r = term.rhs;
-    if (r.start_col < 0 && r.n_steps == 0 && l.start_col >= 0 && cols[l.start_col].dtype == FLOCKGPU_INT32) {
+    if (r.start_col < 0 && r.n_steps == 0 && l.start_col >= 0 && is_i32(cols[l.start_col].dtype)) {
       if (l.n_steps == 0) {
         out.fast.kind = FAST_PRED_I32_CMP;
         out.fast.col = l.start_col;
@@ -800,6 +814,24 @@ struct TreeBuilder {
         }
         break;
       }
+      case FLOCKGPU_OP_LIKE:
+      case FLOCKGPU_OP_NOT_LIKE: {
+        const Node& v = t.nodes[n.l];
+        const Node& pat = t.nodes[n.r];
+        if (v.op == FLOCKGPU_OP_LIT_NULL || pat.op == FLOCKGPU_OP_LIT_NULL) {
+          id = lit_node(Val{0}, true);
+          break;
+        }
+        FG_CHECK(v.op == FLOCKGPU_OP_COLUMN, FLOCKGPU_ERR_UNSUPPORTED, "expression: LIKE needs a column operand");
+        TNode x;
+        x.op = T_LIKE;
+        x.sub = n.op == FLOCKGPU_OP_NOT_LIKE;
+        x.col = v.col;
+        x.may_null = cols[v.col].has_nulls;
+        pooled(pat.s, &x.lit);
+        id = intern(x);
+        break;
+      }
       case FLOCKGPU_OP_IN_LIST: {
         // x IN (a, b) is x = a OR x = b under Kleene's OR: exactly SQL's three-valued IN
         for (size_t k = 1; k < n.kids.size(); ++k) {
@@ -971,7 +1003,8 @@ std::string expr_to_string(const Expr& e, const std::vector<ColInfo>& cols) {
       case FLOCKGPU_OP_DIV: return "/"; case FLOCKGPU_OP_MOD: return "%"; case FLOCKGPU_OP_EQ: return "=";
       case FLOCKGPU_OP_NE: return "!="; case FLOCKGPU_OP_LT: return "<"; case FLOCKGPU_OP_LE: return "<=";
       case FLOCKGPU_OP_GT: return ">"; case FLOCKGPU_OP_GE: return ">="; case FLOCKGPU_OP_AND: return "AND";
-      case FLOCKGPU_OP_OR: return "OR"; default: return "?";
+      case FLOCKGPU_OP_OR: return "OR"; case FLOCKGPU_OP_LIKE: return "LIKE"; case FLOCKGPU_OP_NOT_LIKE: return "NOT LIKE";
+      default: return "?";
     }
   };
   char buf[64];

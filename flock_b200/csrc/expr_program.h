@@ -126,7 +126,7 @@ struct OutCol {
 FG_HD Val load_val(const ColRef& c, int64_t row) {
   Val v;
   switch (c.dtype) {
-    case FLOCKGPU_INT32: v.i = static_cast<const int32_t*>(c.data)[row]; break;
+    case FLOCKGPU_INT32: case FLOCKGPU_DATE32: v.i = static_cast<const int32_t*>(c.data)[row]; break;
     case FLOCKGPU_UINT32: v.u = static_cast<const uint32_t*>(c.data)[row]; break;
     case FLOCKGPU_FLOAT64: v.d = static_cast<const double*>(c.data)[row]; break;
     default: v.i = static_cast<const int64_t*>(c.data)[row]; break;  // Int64 / UInt64 / Timestamp
@@ -136,7 +136,7 @@ FG_HD Val load_val(const ColRef& c, int64_t row) {
 
 FG_HD void store_val(void* dst, int dtype, int64_t pos, Val v) {
   switch (dtype) {
-    case FLOCKGPU_INT32: case FLOCKGPU_UINT32: static_cast<int32_t*>(dst)[pos] = int32_t(v.i); break;
+    case FLOCKGPU_INT32: case FLOCKGPU_UINT32: case FLOCKGPU_DATE32: static_cast<int32_t*>(dst)[pos] = int32_t(v.i); break;
     case FLOCKGPU_FLOAT64: static_cast<double*>(dst)[pos] = v.d; break;
     default: static_cast<int64_t*>(dst)[pos] = v.i; break;
   }

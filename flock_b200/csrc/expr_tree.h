@@ -37,7 +37,8 @@ enum TreeOp : int16_t {
   T_NOT,
   T_IS_NULL, T_IS_NOT_NULL,
   T_SELECT,       // r[d] = r[c] is TRUE ? r[a] : r[b]   (a NULL condition takes r[b]: CASE falls through)
-  T_STORE         // output `col` = r[a]
+  T_STORE,        // output `col` = r[a]
+  T_LIKE          // r[d] = Utf8 column `col` LIKE pooled pattern lit (offset << 32 | length); sub = 1: NOT LIKE
 };
 
 constexpr uint8_t TF_NULL = 1, TF_ERR = 2;
@@ -73,6 +74,38 @@ struct TreeRegs {
   FG_HD uint8_t& flag(int reg, int j) const { return f[(reg * R + j) * STRIDE]; }
 };
 
+// SQL LIKE without an escape character: '%' matches any run of characters, '_' exactly one UTF-8 code point, every
+// other byte itself.  Greedy two-pointer match that backtracks to the last '%' only, so it needs no stack: the
+// pattern up to that '%' is already matched, and a later '%' makes every earlier choice final.
+FG_HD int next_code_point(const uint8_t* s, int i, int n) {
+  ++i;
+  while (i < n && (s[i] & 0xc0) == 0x80) ++i;
+  return i;
+}
+
+FG_HD bool like_match(const uint8_t* s, int n, const uint8_t* p, int m) {
+  int si = 0, pi = 0, star = -1, mark = 0;
+  while (si < n) {
+    if (pi < m && p[pi] == '%') {
+      star = ++pi;
+      mark = si;
+    } else if (pi < m && p[pi] == '_') {
+      ++pi;
+      si = next_code_point(s, si, n);
+    } else if (pi < m && p[pi] == s[si]) {
+      ++pi;
+      ++si;
+    } else if (star >= 0) {
+      pi = star;
+      si = mark = next_code_point(s, mark, n);
+    } else {
+      return false;
+    }
+  }
+  while (pi < m && p[pi] == '%') ++pi;
+  return pi == m;
+}
+
 // Runs the program for R rows (rows[j] < 0: no row); returns bit j = the verdict register is TRUE for row j.
 // `vec`: rows[0..4) are four consecutive rows starting at a multiple of four (R == 4): fixed-width columns are
 // read and results written 16 bytes at a time where the buffers are aligned.
@@ -87,7 +120,7 @@ FG_HD unsigned eval_tree(const TreeProgram& p, const ColRef* cols, const TreeOut
         bool done = false;
 #ifdef __CUDA_ARCH__
         if (R == 4 && vec && col.dtype != FLOCKGPU_UTF8) {
-          const int w = (col.dtype == FLOCKGPU_INT32 || col.dtype == FLOCKGPU_UINT32) ? 4 : 8;
+          const int w = (col.dtype == FLOCKGPU_INT32 || col.dtype == FLOCKGPU_UINT32 || col.dtype == FLOCKGPU_DATE32) ? 4 : 8;
           const char* src = static_cast<const char*>(col.data) + rows[0] * w;
           if ((reinterpret_cast<uintptr_t>(src) & 15) == 0) {
             if (w == 4) {
@@ -96,7 +129,7 @@ FG_HD unsigned eval_tree(const TreeProgram& p, const ColRef* cols, const TreeOut
 #pragma unroll
               for (int j = 0; j < R; ++j) {
                 Val v;
-                if (col.dtype == FLOCKGPU_INT32) v.i = xs[j];
+                if (col.dtype != FLOCKGPU_UINT32) v.i = xs[j];
                 else v.u = uint32_t(xs[j]);
                 rf.val(in.d, j) = v;
               }
@@ -190,6 +223,25 @@ FG_HD unsigned eval_tree(const TreeProgram& p, const ColRef* cols, const TreeOut
         }
         break;
       }
+      case T_LIKE: {
+        const ColRef c = cols[in.col];
+        const uint8_t* pat = reinterpret_cast<const uint8_t*>(p.pool) + (in.lit.u >> 32);
+        const int np = int(in.lit.u & 0xffffffffu);
+#pragma unroll
+        for (int j = 0; j < R; ++j) {
+          Val v;
+          v.i = 0;
+          uint8_t f = TF_NULL;
+          if (rows[j] >= 0 && !(c.validity && !c.validity[rows[j]])) {
+            f = 0;
+            const int32_t lo = c.offsets[rows[j]], hi = c.offsets[rows[j] + 1];
+            v.i = int64_t(like_match(static_cast<const uint8_t*>(c.data) + lo, hi - lo, pat, np) != (in.sub != 0));
+          }
+          rf.val(in.d, j) = v;
+          rf.flag(in.d, j) = f;
+        }
+        break;
+      }
       case T_AND:
       case T_OR:
 #pragma unroll
@@ -247,7 +299,7 @@ FG_HD unsigned eval_tree(const TreeProgram& p, const ColRef* cols, const TreeOut
 #ifdef __CUDA_ARCH__
         if (R == 4 && vec) {
           // rows[0] is a multiple of four and output buffers are fresh allocations: 16-byte aligned stores
-          if (o.dtype == FLOCKGPU_INT32 || o.dtype == FLOCKGPU_UINT32) {
+          if (o.dtype == FLOCKGPU_INT32 || o.dtype == FLOCKGPU_UINT32 || o.dtype == FLOCKGPU_DATE32) {
             int4 x;
             x.x = int32_t(rf.val(in.a, 0).i); x.y = int32_t(rf.val(in.a, 1 % R).i);
             x.z = int32_t(rf.val(in.a, 2 % R).i); x.w = int32_t(rf.val(in.a, 3 % R).i);

@@ -1151,6 +1151,119 @@ __global__ void __launch_bounds__(256) agg_insert_rows_kernel(const __grid_const
   if ((threadIdx.x & 31) == 0 && claimed) atomicAdd(a.n_groups, (unsigned long long)claimed);
 }
 
+// ---- level 1 for row keys: CTA-local pre-aggregation (TPC-H q1: ~6 M rows per SF into 4 (Utf8, Utf8) groups, where
+// agg_insert_rows_kernel would send every thread of the GPU to the same four slots).  Each CTA owns a contiguous row
+// range and keeps an open-addressing table of RL_SLOTS slots in shared memory: one 64-bit word (hash tag << 32 | the
+// group's representative row) and one accumulator per aggregate.  A probe compares the tag first, then the key columns
+// (rows_equal).  Lanes of a warp that land on the same slot combine their values first (__match_any_sync on the slot,
+// then the leader folds its peers' values in), so a warp step costs one shared atomic per distinct slot and
+// accumulator.  Before a tile could take the table past 3/4 full, and at the end, the CTA merges its entries into the
+// level-2 row table (agg_insert_rows_kernel's table, keyed by representative row) with the merge operation of each
+// accumulator; agg_emit_kernel<2> then runs unchanged.
+constexpr int RL_SLOTS = 1024;
+constexpr int RL_THREADS = 256;
+constexpr unsigned long long RL_EMPTY = ~0ull;
+
+__device__ __forceinline__ void rows_table_merge(const AggRowsArgs& a, unsigned rep, const unsigned long long* s_acc, int s, unsigned* claimed) {
+  unsigned long long slot = hash_row(a.keys, a.cols, rep) & (a.cap - 1);
+  while (true) {
+    unsigned cur = a.owner[slot];
+    if (cur == EMPTY_OWNER) {
+      cur = atomicCAS(&a.owner[slot], EMPTY_OWNER, rep);
+      if (cur == EMPTY_OWNER) {
+        ++*claimed;
+        break;
+      }
+    }
+    if (rows_equal(a.keys, a.cols, int64_t(cur), a.keys, a.cols, rep)) break;
+    slot = (slot + 1) & (a.cap - 1);
+  }
+  for (int c = 0; c < a.n_acc; ++c) {
+    Val v;
+    v.u = s_acc[c * RL_SLOTS + s];
+    acc_apply(&a.tacc[c * a.cap + slot], acc_merge_op(a.acc[c].op), v);
+  }
+}
+
+__global__ void __launch_bounds__(RL_THREADS) agg_rows_local_kernel(const __grid_constant__ AggRowsArgs a, int64_t rows_per_cta) {
+  extern __shared__ unsigned long long rl_smem[];
+  unsigned long long* s_word = rl_smem;              // [RL_SLOTS]
+  unsigned long long* s_acc = rl_smem + RL_SLOTS;    // [n_acc][RL_SLOTS]
+  const int lane = threadIdx.x & 31;
+  for (int s = threadIdx.x; s < RL_SLOTS; s += blockDim.x) {
+    s_word[s] = RL_EMPTY;
+    for (int c = 0; c < a.n_acc; ++c) s_acc[c * RL_SLOTS + s] = acc_identity(a.acc[c].op);
+  }
+  __syncthreads();
+  unsigned claimed = 0;
+  int used = 0;  // slots in use, the same in every thread (__syncthreads_count)
+  auto flush = [&]() {
+    __syncthreads();
+    for (int s = threadIdx.x; s < RL_SLOTS; s += blockDim.x) {
+      const unsigned long long w = s_word[s];
+      if (w == RL_EMPTY) continue;
+      rows_table_merge(a, unsigned(w), s_acc, s, &claimed);
+      s_word[s] = RL_EMPTY;
+      for (int c = 0; c < a.n_acc; ++c) s_acc[c * RL_SLOTS + s] = acc_identity(a.acc[c].op);
+    }
+    used = 0;
+    __syncthreads();
+  };
+  const int64_t begin = int64_t(blockIdx.x) * rows_per_cta;
+  const int64_t end = begin + rows_per_cta < a.n_rows ? begin + rows_per_cta : a.n_rows;
+  for (int64_t base = begin; base < end; base += RL_THREADS) {
+    // a tile claims at most RL_THREADS slots: flush first when that could pass 3/4 of the table
+    if (used + RL_THREADS > RL_SLOTS * 3 / 4) flush();
+    const int64_t row = base + threadIdx.x;
+    const bool live = row < end;
+    unsigned slot = 0xffffffffu;
+    bool new_slot = false;
+    if (live) {
+      const unsigned long long h = hash_row(a.keys, a.cols, row);
+      const unsigned long long mine = ((h >> 32) << 32) | (unsigned long long)unsigned(row);
+      unsigned s = unsigned(h) & (RL_SLOTS - 1);
+      while (true) {
+        unsigned long long w = s_word[s];
+        if (w == RL_EMPTY) {
+          w = atomicCAS(&s_word[s], RL_EMPTY, mine);
+          if (w == RL_EMPTY) {
+            new_slot = true;
+            break;
+          }
+        }
+        if ((w >> 32) == (h >> 32) && rows_equal(a.keys, a.cols, int64_t(unsigned(w)), a.keys, a.cols, row)) break;
+        s = (s + 1) & (RL_SLOTS - 1);
+      }
+      slot = s;
+    }
+    const unsigned peers = __match_any_sync(FULL_MASK, slot);
+    const int leader = __ffs(peers) - 1;
+    // lanes whose value a leader folds in: every live lane that is not its group's leader (warp-uniform)
+    const unsigned others = __ballot_sync(FULL_MASK, live && lane != leader);
+    for (int c = 0; c < a.n_acc; ++c) {
+      const AccDesc d = a.acc[c];
+      const int op = d.op == ACC_COUNT ? ACC_ADD_I : d.op;  // a count adds 1 per row with a non-NULL argument
+      Val v;
+      v.u = acc_identity(op);
+      if (live && acc_input_valid(d, a.cols, row)) {
+        if (d.op == ACC_COUNT) v.u = 1;
+        else v = load_acc_input(d, a.cols, row);
+      }
+      for (unsigned m = others; m; m &= m - 1) {
+        const int k = __ffs(m) - 1;
+        Val o;
+        o.u = __shfl_sync(FULL_MASK, v.u, k);
+        if (lane == leader && ((peers >> k) & 1u)) v = acc_combine(op, v, o);
+      }
+      if (live && lane == leader) acc_apply(&s_acc[c * RL_SLOTS + slot], op, v);
+    }
+    used += __syncthreads_count(new_slot);
+  }
+  flush();
+  claimed = warp_sum(claimed);
+  if (lane == 0 && claimed) atomicAdd(a.n_groups, (unsigned long long)claimed);
+}
+
 // ================================================================================================
 // emit: compaction of the occupied slots
 // ================================================================================================
@@ -1300,7 +1413,7 @@ __global__ void __launch_bounds__(CP_THREADS) agg_emit_kernel(const __grid_const
               if ((nib >> e) & 1u) d.valid_dst[pos[e]] = pv[e] != 0ull;
           }
           // one uniform width branch per column instead of a type switch per element
-          if (d.out_dtype == FLOCKGPU_INT32 || d.out_dtype == FLOCKGPU_UINT32) {
+          if (d.out_dtype == FLOCKGPU_INT32 || d.out_dtype == FLOCKGPU_UINT32 || d.out_dtype == FLOCKGPU_DATE32) {
 #pragma unroll
             for (int e = 0; e < 4; ++e)
               if ((nib >> e) & 1u) static_cast<uint32_t*>(d.dst)[pos[e]] = uint32_t(v[e].u);
@@ -1384,7 +1497,7 @@ __global__ void agg_emit_one_kernel(const __grid_constant__ AggEmitOneArgs a) {
 namespace {
 
 bool is_unsigned_dt(int dt) { return dt == FLOCKGPU_UINT32 || dt == FLOCKGPU_UINT64; }
-bool is_signed_dt(int dt) { return dt == FLOCKGPU_INT32 || dt == FLOCKGPU_INT64 || dt == FLOCKGPU_TIMESTAMP; }
+bool is_signed_dt(int dt) { return dt == FLOCKGPU_INT32 || dt == FLOCKGPU_INT64 || dt == FLOCKGPU_TIMESTAMP || dt == FLOCKGPU_DATE32; }
 
 struct OutPlan {
   std::string name;
@@ -1426,11 +1539,11 @@ AggPlan plan_aggregates(const Table& in, int mode, const std::vector<AggSpec>& a
   const bool from_states = mode == FLOCKGPU_AGG_FINAL || mode == FLOCKGPU_AGG_FINAL_PARTITIONED;
   const bool partial_out = mode == FLOCKGPU_AGG_PARTIAL;
   auto add_acc = [&](int op, int col, int cvt) {
-    // "how many non-NULL values of column c" is wanted by COUNT(c) and by the validity of SUM / MIN / MAX / AVG over c:
-    // one accumulator serves them all
-    if (op == ACC_COUNT && col >= 0)
-      for (size_t i = 0; i < accs->size(); ++i)
-        if ((*accs)[i].op == ACC_COUNT && (*accs)[i].col == col && (*accs)[i].cvt == cvt) return int(i);
+    // identical accumulators are one: "how many non-NULL values of column c" is wanted by COUNT(c) and by the validity
+    // of SUM / MIN / MAX / AVG over c, COUNT(*) by every AVG over a non-nullable column, SUM(x) by AVG(x) (TPC-H q1's
+    // eleven accumulators are six)
+    for (size_t i = 0; i < accs->size(); ++i)
+      if ((*accs)[i].op == op && (*accs)[i].col == col && (*accs)[i].cvt == cvt) return int(i);
     FG_CHECK(accs->size() < size_t(MAX_ACC), FLOCKGPU_ERR_UNSUPPORTED, "hash_aggregate: more than %d accumulators", MAX_ACC);
     accs->push_back(AccDesc{op, col, cvt, 0});
     return int(accs->size()) - 1;
@@ -1487,7 +1600,7 @@ AggPlan plan_aggregates(const Table& in, int mode, const std::vector<AggSpec>& a
           a_sum = add_acc(ACC_ADD_F, s.col + 1, CVT_NONE);
         } else {
           int dt = col_dtype(s.col, "AVG");
-          FG_CHECK(dt != FLOCKGPU_UTF8 && dt != FLOCKGPU_TIMESTAMP, FLOCKGPU_ERR_UNSUPPORTED, "hash_aggregate: AVG over %s", dtype_name(dt));
+          FG_CHECK(dt != FLOCKGPU_UTF8 && dt != FLOCKGPU_TIMESTAMP && dt != FLOCKGPU_DATE32, FLOCKGPU_ERR_UNSUPPORTED, "hash_aggregate: AVG over %s", dtype_name(dt));
           a_cnt = add_acc(ACC_COUNT, nulls_in(s.col) ? s.col : -1, CVT_NONE);  // AVG divides by the number of non-NULL values
           a_sum = add_acc(ACC_ADD_F, s.col, dt == FLOCKGPU_FLOAT64 ? CVT_NONE : (is_unsigned_dt(dt) ? CVT_U2F : CVT_I2F));
         }
@@ -2352,7 +2465,11 @@ static GroupTable packed_table(const CtxPtr& ctx, const Table& in, const KeyPack
 
 // ---- Utf8, wide or nullable keys: a table of representative input rows (key equality against the input columns).
 // Returns the result itself when a DISTINCT finds every row different, else NULL with `t` ready to be emitted.
-static TablePtr row_table(const CtxPtr& ctx, const Table& in, const std::vector<int>& group_cols, const AggPlan& p, GroupTable* t) {
+// agg_rows_local_kernel is taken when at least this share of a 64 Ki-row sample repeats an earlier key of the sample
+constexpr double ROWS_LOCAL_MIN_DUPLICATES = 0.5;
+
+static TablePtr row_table(const CtxPtr& ctx, const TablePtr& in_ptr, const std::vector<int>& group_cols, const AggPlan& p, GroupTable* t) {
+  const Table& in = *in_ptr;
   FG_CHECK(group_cols.size() <= size_t(MAX_KEY_COLS), FLOCKGPU_ERR_UNSUPPORTED, "hash_aggregate: more than %d group columns", MAX_KEY_COLS);
   const int64_t n = in.num_rows;
   const int n_acc = p.n_acc();
@@ -2410,7 +2527,16 @@ static TablePtr row_table(const CtxPtr& ctx, const Table& in, const std::vector<
   ra.cap = cap;
   ra.n_groups = ctx->d_scalars + 7;
   FG_CUDA(cudaMemsetAsync(ra.n_groups, 0, 8, ctx->stream));
-  {
+  // Mostly repeated keys over a large input (TPC-H q1, q5 and q12 at scale): pre-aggregate per CTA first.  The cut-off
+  // (DESIGN.md K6r) keeps inputs whose keys are mostly distinct, and small ones, on the direct insert.
+  if (n >= (int64_t(1) << 18) && n < int64_t(EMPTY_OWNER) && distinct_sample_duplicates(ctx, in_ptr, group_cols) >= ROWS_LOCAL_MIN_DUPLICATES) {
+    const size_t smem = size_t(RL_SLOTS) * 8 * (1 + n_acc);
+    FG_CUDA(cudaFuncSetAttribute(agg_rows_local_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+    const int grid = resident_grid(ctx, reinterpret_cast<const void*>(agg_rows_local_kernel), RL_THREADS, smem, n, RL_THREADS * 16);
+    const int64_t per_cta = ((n + grid - 1) / grid + RL_THREADS - 1) / RL_THREADS * RL_THREADS;
+    LaunchTimer lt(ctx, "agg_rows_local_kernel");
+    agg_rows_local_kernel<<<grid, RL_THREADS, smem, ctx->stream>>>(ra, per_cta);
+  } else {
     LaunchTimer lt(ctx, "agg_insert_rows_kernel");
     agg_insert_rows_kernel<<<grid_for(ctx, n, 256, 8), 256, 0, ctx->stream>>>(ra);
   }
@@ -2650,7 +2776,7 @@ static TablePtr hash_aggregate_impl(const CtxPtr& ctx, const TablePtr& in_ptr, i
     // when tried, the dense table overflowed and the stage paid both paths)
     Partials l1;
     if (n >= (int64_t(1) << 18) && size_t(AL_SLOTS) * 8 * (1 + n_acc) <= 200 * 1024 && !states_in) {
-      const bool count32 = kp.n == 1 && kp.width[0] == 4 && (n_acc == 0 || (n_acc == 1 && p.accs[0].op == ACC_COUNT && p.accs[0].col < 0));
+      const bool count32 = kp.n == 1 && kp.width[0] == 4 && p.outs.size() <= 1 && (n_acc == 0 || (n_acc == 1 && p.accs[0].op == ACC_COUNT && p.accs[0].col < 0));
       if (count32 && allow_dense && n < (int64_t(1) << 32)) return count_table(ctx, in_ptr, mode, group_cols, aggs, p);
       l1 = level1_partials(ctx, in, kp, p, count32);
     }
@@ -2671,7 +2797,7 @@ static TablePtr hash_aggregate_impl(const CtxPtr& ctx, const TablePtr& in_ptr, i
       }
       return groups_table(core, kinds, names, in.metadata);
     }
-  } else if (TablePtr distinct = row_table(ctx, in, group_cols, p, &t)) {
+  } else if (TablePtr distinct = row_table(ctx, in_ptr, group_cols, p, &t)) {
     return distinct;
   }
   return emit_groups(ctx, in, group_cols, p, t);

@@ -26,6 +26,7 @@ static void parse_data_type(const Json& j, int* dtype, std::string* format) {
     if (s == "UInt64") { *dtype = FLOCKGPU_UINT64; *format = "L"; return; }
     if (s == "Float64") { *dtype = FLOCKGPU_FLOAT64; *format = "g"; return; }
     if (s == "Utf8") { *dtype = FLOCKGPU_UTF8; *format = "u"; return; }
+    if (s == "Date32") { *dtype = FLOCKGPU_DATE32; *format = "tdD"; return; }
     fail(FLOCKGPU_ERR_UNSUPPORTED, "plan JSON: data type %s is not supported on the GPU path", s.c_str());
   }
   if (j.is_object()) {
@@ -91,6 +92,30 @@ static bool is_column_expr(const Json& e) {
   return k && k->is_string() && k->str == "column";
 }
 
+// Days since 1970-01-01 of a proleptic Gregorian 'YYYY-MM-DD' (what CAST('1998-09-02' AS DATE) reads).
+static int64_t parse_date32(const std::string& s) {
+  auto digits = [&](size_t at, size_t n) {
+    int v = 0;
+    for (size_t i = at; i < at + n; ++i) {
+      if (s[i] < '0' || s[i] > '9') fail(FLOCKGPU_ERR_INVALID, "plan: \"%s\" is not a date (YYYY-MM-DD)", s.c_str());
+      v = v * 10 + (s[i] - '0');
+    }
+    return v;
+  };
+  if (s.size() != 10 || s[4] != '-' || s[7] != '-') fail(FLOCKGPU_ERR_INVALID, "plan: \"%s\" is not a date (YYYY-MM-DD)", s.c_str());
+  const int y = digits(0, 4), m = digits(5, 2), d = digits(8, 2);
+  const bool leap = (y % 4 == 0 && y % 100 != 0) || y % 400 == 0;
+  static const int month_days[12] = {31, 28, 31, 30, 31, 30, 31, 31, 30, 31, 30, 31};
+  if (m < 1 || m > 12 || d < 1 || d > month_days[m - 1] + (m == 2 && leap))
+    fail(FLOCKGPU_ERR_INVALID, "plan: \"%s\" is not a date (YYYY-MM-DD)", s.c_str());
+  // days_from_civil (H. Hinnant): eras of 400 years starting in March
+  const int yy = m <= 2 ? y - 1 : y;
+  const int era = (yy >= 0 ? yy : yy - 399) / 400, yoe = yy - era * 400;
+  const int doy = (153 * (m + (m > 2 ? -3 : 9)) + 2) / 5 + d - 1;
+  const int doe = yoe * 365 + yoe / 4 - yoe / 100 + doy;
+  return int64_t(era) * 146097 + doe - 719468;
+}
+
 static ExprTok scalar_token(const Json& value) {
   if (!value.is_object() || value.obj.size() != 1) fail(FLOCKGPU_ERR_INVALID, "plan JSON: malformed ScalarValue");
   const std::string& ty = value.obj[0].first;
@@ -100,13 +125,18 @@ static ExprTok scalar_token(const Json& value) {
     t.op = FLOCKGPU_OP_LIT_NULL;
     t.dtype = ty == "Float64" || ty == "Float32" ? FLOCKGPU_FLOAT64 : ty == "Utf8" || ty == "LargeUtf8" ? FLOCKGPU_UTF8 : ty == "Boolean" ? FLOCKGPU_BOOL
               : ty == "Int32" ? FLOCKGPU_INT32 : ty == "UInt32" ? FLOCKGPU_UINT32 : ty == "UInt64" ? FLOCKGPU_UINT64
-              : ty.rfind("Timestamp", 0) == 0 ? FLOCKGPU_TIMESTAMP : FLOCKGPU_INT64;
+              : ty.rfind("Timestamp", 0) == 0 ? FLOCKGPU_TIMESTAMP : ty == "Date32" ? FLOCKGPU_DATE32 : FLOCKGPU_INT64;
     return t;
   }
   if (ty == "Float64" || ty == "Float32") {
     t.op = FLOCKGPU_OP_LIT_F64;
     t.dtype = FLOCKGPU_FLOAT64;
     t.f64 = v.num;
+  } else if (ty == "Date32") {
+    t.op = FLOCKGPU_OP_LIT_I64;
+    t.dtype = FLOCKGPU_DATE32;
+    t.i64 = v.as_int("Date32 literal");
+    if (t.i64 < INT32_MIN || t.i64 > INT32_MAX) fail(FLOCKGPU_ERR_INVALID, "plan: Date32 literal %lld out of range", (long long)t.i64);
   } else if (ty == "Utf8" || ty == "LargeUtf8") {
     t.op = FLOCKGPU_OP_LIT_UTF8;
     t.dtype = FLOCKGPU_UTF8;
@@ -127,7 +157,8 @@ static int binary_op(const std::string& op) {
   static const std::pair<const char*, int> table[] = {
       {"Eq", FLOCKGPU_OP_EQ}, {"NotEq", FLOCKGPU_OP_NE}, {"Lt", FLOCKGPU_OP_LT}, {"LtEq", FLOCKGPU_OP_LE}, {"Gt", FLOCKGPU_OP_GT},
       {"GtEq", FLOCKGPU_OP_GE}, {"Plus", FLOCKGPU_OP_ADD}, {"Minus", FLOCKGPU_OP_SUB}, {"Multiply", FLOCKGPU_OP_MUL},
-      {"Divide", FLOCKGPU_OP_DIV}, {"Modulo", FLOCKGPU_OP_MOD}, {"Modulus", FLOCKGPU_OP_MOD}, {"And", FLOCKGPU_OP_AND}, {"Or", FLOCKGPU_OP_OR}};
+      {"Divide", FLOCKGPU_OP_DIV}, {"Modulo", FLOCKGPU_OP_MOD}, {"Modulus", FLOCKGPU_OP_MOD}, {"And", FLOCKGPU_OP_AND}, {"Or", FLOCKGPU_OP_OR},
+      {"Like", FLOCKGPU_OP_LIKE}, {"NotLike", FLOCKGPU_OP_NOT_LIKE}};
   for (const auto& kv : table)
     if (op == kv.first) return kv.second;
   fail(FLOCKGPU_ERR_UNSUPPORTED, "plan: binary operator %s", op.c_str());
@@ -143,7 +174,22 @@ static void emit_expr(const Json& e, const fg::Table& in, Expr* out) {
   } else if (kind == "literal") {
     out->push_back(scalar_token(e.at("value")));
   } else if (kind == "cast_expr" || kind == "try_cast_expr") {
-    emit_expr(e.at("expr"), in, out);
+    // CAST('YYYY-MM-DD' AS Date32), the form of SQL's DATE 'YYYY-MM-DD' before constant folding, becomes a Date32
+    // literal here; every other cast to or from Date32 is refused by the expression compiler
+    const Json& inner = e.at("expr");
+    const Json& ct = e.at("cast_type");
+    const Json* lk = inner.get("physical_expr");
+    const Json* lv = inner.get("value");
+    if (ct.is_string() && ct.str == "Date32" && lk && lk->is_string() && lk->str == "literal" && lv && lv->is_object() && lv->obj.size() == 1 &&
+        (lv->obj[0].first == "Utf8" || lv->obj[0].first == "LargeUtf8") && lv->obj[0].second->is_string()) {
+      ExprTok t{};
+      t.op = FLOCKGPU_OP_LIT_I64;
+      t.dtype = FLOCKGPU_DATE32;
+      t.i64 = parse_date32(lv->obj[0].second->str);
+      out->push_back(t);
+      return;
+    }
+    emit_expr(inner, in, out);
     ExprTok t{};
     t.op = FLOCKGPU_OP_CAST;
     std::string fmt;
@@ -237,6 +283,40 @@ static std::vector<int> expr_columns(const ExecEnv& env, TablePtr* in, const std
   return cols;
 }
 
+static void column_refs(const Json& e, std::vector<const Json*>* out) {
+  if (is_column_expr(e)) {
+    out->push_back(&e);
+  } else if (e.is_object()) {
+    for (const auto& kv : e.obj) column_refs(*kv.second, out);
+  } else if (e.is_array()) {
+    for (const JsonPtr& x : e.arr) column_refs(*x, out);
+  }
+}
+
+// *in reduced to the columns `exprs` read, in input order (views: nothing is copied), when every reference still
+// resolves to the same column.  An aggregate over a join sees every column of both sides, more than one kernel
+// argument block holds (TPC-H q5 and q10), while its expressions read a handful.
+static void narrow_input(const std::vector<const Json*>& exprs, TablePtr* in) {
+  const fg::Table& full = **in;
+  full.resolve();
+  std::vector<const Json*> refs;
+  for (const Json* e : exprs)
+    if (e) column_refs(*e, &refs);
+  std::vector<int> at(full.cols.size(), -1);
+  for (const Json* r : refs) at[column_of(*r, full)] = 0;
+  auto narrow = std::make_shared<fg::Table>(full);
+  narrow->cols.clear();
+  for (size_t c = 0; c < full.cols.size(); ++c)
+    if (at[c] == 0) {
+      at[c] = int(narrow->cols.size());
+      narrow->cols.push_back(full.cols[c]);
+    }
+  if (narrow->cols.empty() || narrow->cols.size() == full.cols.size()) return;
+  for (const Json* r : refs)
+    if (resolve_column(*narrow, r->at("name").as_string("column name"), -1) != at[column_of(*r, full)]) return;  // ambiguous names
+  *in = narrow;
+}
+
 // Group columns and aggregate arguments of a Partial / Single aggregate over *in (COUNT over a literal is COUNT(*): -1).
 static void aggregate_columns(const ExecEnv& env, const HashAggregateExec& n, TablePtr* in, std::vector<int>* gcols, std::vector<int>* acols) {
   std::vector<const Json*> exprs;
@@ -246,6 +326,7 @@ static void aggregate_columns(const ExecEnv& env, const HashAggregateExec& n, Ta
     const bool literal = k && k->is_string() && k->str == "literal";
     exprs.push_back(a.func == FLOCKGPU_AGG_COUNT && literal ? nullptr : a.expr);
   }
+  narrow_input(exprs, in);
   const std::vector<int> cols = expr_columns(env, in, exprs);
   gcols->assign(cols.begin(), cols.begin() + n.group_expr.size());
   acols->assign(cols.begin() + n.group_expr.size(), cols.end());
@@ -288,7 +369,8 @@ static std::string expr_display(const Json& e) {
   if (kind == "binary_expr") {
     static const std::pair<const char*, const char*> sym[] = {{"Eq", "="}, {"NotEq", "!="}, {"Lt", "<"}, {"LtEq", "<="}, {"Gt", ">"},
                                                                {"GtEq", ">="}, {"Plus", "+"}, {"Minus", "-"}, {"Multiply", "*"}, {"Divide", "/"},
-                                                               {"Modulo", "%"}, {"Modulus", "%"}, {"And", "AND"}, {"Or", "OR"}};
+                                                               {"Modulo", "%"}, {"Modulus", "%"}, {"And", "AND"}, {"Or", "OR"},
+                                                               {"Like", "LIKE"}, {"NotLike", "NOT LIKE"}};
     std::string op = e.at("op").str;
     for (const auto& kv : sym)
       if (op == kv.first) op = kv.second;

@@ -471,7 +471,8 @@ TablePtr import_ndjson(const CtxPtr& ctx, const ArrowSchema* schema, const uint8
   for (int c = 0; c < n_cols; ++c) {
     const ArrowSchema* cs = schema->children[c];
     const int dt = dtype_from_format(cs->format);
-    FG_CHECK(dt >= 0 && dt != FLOCKGPU_BOOL, FLOCKGPU_ERR_UNSUPPORTED, "table_import_ndjson: column \"%s\" has unsupported Arrow format \"%s\"", cs->name ? cs->name : "",
+    // Date32 in NDJSON (date strings) is not parsed
+    FG_CHECK(dt >= 0 && dt != FLOCKGPU_BOOL && dt != FLOCKGPU_DATE32, FLOCKGPU_ERR_UNSUPPORTED, "table_import_ndjson: column \"%s\" has unsupported Arrow format \"%s\"", cs->name ? cs->name : "",
              cs->format ? cs->format : "");
     const int len = int(strlen(cs->name ? cs->name : ""));
     FG_CHECK(pool + len <= NJ_NAME_POOL, FLOCKGPU_ERR_UNSUPPORTED, "table_import_ndjson: field names exceed %d bytes", NJ_NAME_POOL);

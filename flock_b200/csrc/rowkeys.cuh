@@ -14,7 +14,7 @@
 
 namespace fg {
 
-constexpr int MAX_KEY_COLS = 4;
+constexpr int MAX_KEY_COLS = 8;
 
 struct KeyPack {
   int32_t n;         // 1 or 2 columns

@@ -45,6 +45,7 @@ __device__ __forceinline__ unsigned long long sortable_u64(const ColRef& c, int6
   }
   switch (c.dtype) {
     case FLOCKGPU_INT32:
+    case FLOCKGPU_DATE32:
       k = (unsigned long long)(static_cast<const uint32_t*>(c.data)[row] ^ 0x80000000u);
       mask = 0xffffffffull;
       break;
@@ -210,7 +211,7 @@ struct RowNumberArgs {
 __device__ __forceinline__ bool same_partition(const RowNumberArgs& a, int64_t i, int64_t j) {
   for (int k = 0; k < a.n_keys; ++k) {
     const ColRef& c = a.key[k];
-    if (c.dtype == FLOCKGPU_INT32 || c.dtype == FLOCKGPU_UINT32) {
+    if (c.dtype == FLOCKGPU_INT32 || c.dtype == FLOCKGPU_UINT32 || c.dtype == FLOCKGPU_DATE32) {
       if (static_cast<const uint32_t*>(c.data)[i] != static_cast<const uint32_t*>(c.data)[j]) return false;
     } else if (static_cast<const unsigned long long*>(c.data)[i] != static_cast<const unsigned long long*>(c.data)[j]) {
       return false;

@@ -11,7 +11,7 @@ from __future__ import annotations
 
 import pyarrow as pa
 
-from . import nexgen, ysbgen
+from . import nexgen, tpchgen, ysbgen
 
 TARGET_PARTITIONS = 8     # flock/src/configs/flock.toml:113
 TARGET_BATCH_SIZE = 4096  # CoalesceBatchesExec default seen in every plan dump
@@ -25,6 +25,7 @@ def data_type_json(t: pa.DataType):
     if pa.types.is_uint64(t): return "UInt64"
     if pa.types.is_float64(t): return "Float64"
     if pa.types.is_string(t): return "Utf8"
+    if pa.types.is_date32(t): return "Date32"
     if pa.types.is_timestamp(t):
         unit = {"s": "Second", "ms": "Millisecond", "us": "Microsecond", "ns": "Nanosecond"}[t.unit]
         return {"Timestamp": [unit, t.tz]}
@@ -432,3 +433,184 @@ def ysb(n: int = TARGET_PARTITIONS) -> dict:
 
 YSB_QUERIES = {"ysb": ysb}
 YSB_SOURCES = {"ysb": ["ad_event", "campaign"]}
+
+
+# ---- TPC-H (flock/src/datasource/tpch/queries/qN.sql) over Flock's schemas (flock/src/datasource/tpch/mod.rs) -----------
+# The reference ships no TPC-H plan dump, so the shape is DataFusion 6's usual one and unverified: MemoryExec
+# projections -> FilterExec -> Hash repartitions -> Partitioned inner joins in FROM order (keys from the WHERE
+# equalities) -> Partial / FinalPartitioned aggregate -> ProjectionExec -> SortExec.  DATE 'YYYY-MM-DD' is written as
+# CAST('YYYY-MM-DD' AS Date32), the form before constant folding; the plan reader folds it to a Date32 literal.
+class _Rel:
+    """A plan node and the names of its output columns, so that expressions can refer to columns by name."""
+
+    def __init__(self, plan: dict, names: list[str]):
+        self.plan, self.names = plan, names
+
+    def c(self, name: str) -> dict:
+        return column(name, self.names.index(name))
+
+
+def _tpch_scan(table: str, cols: list[str], n: int) -> _Rel:
+    sch = tpchgen.schema(table)
+    return _Rel(repartition_rr(memory_exec(sch, [sch.get_field_index(c) for c in cols]), n), cols)
+
+
+def _date(iso: str) -> dict:
+    return cast(literal("Utf8", iso), "Date32")
+
+
+def _f64(x) -> dict:
+    return cast(literal("Int64", x), "Float64")
+
+
+def _filter(r: _Rel, pred) -> _Rel:
+    return _Rel(coalesce_batches_exec(filter_exec(pred(r), r.plan)), r.names)
+
+
+def _and(*terms: dict) -> dict:
+    out = terms[0]
+    for t in terms[1:]:
+        out = binary(out, "And", t)
+    return out
+
+
+def _join(left: _Rel, right: _Rel, on: list[tuple[str, str]], n: int) -> _Rel:
+    lsh = coalesce_batches_exec(repartition_hash(left.plan, [left.c(a) for a, _ in on], n))
+    rsh = coalesce_batches_exec(repartition_hash(right.plan, [right.c(b) for _, b in on], n))
+    return _Rel(coalesce_batches_exec(hash_join_exec(lsh, rsh, [(left.c(a), right.c(b)) for a, b in on])), left.names + right.names)
+
+
+def _revenue(r: _Rel) -> dict:
+    return binary(r.c("l_extendedprice"), "Multiply", binary(_f64(1), "Minus", r.c("l_discount")))
+
+
+def _grouped(r: _Rel, group: list[str], aggrs: list[dict], n: int) -> _Rel:
+    out = two_phase_aggregate([(g, r.names.index(g)) for g in group], aggrs, r.plan, n)
+    return _Rel(out, group + [a["name"] for a in aggrs])
+
+
+def _project_sort(r: _Rel, exprs: list[tuple[dict, str]], order: list[tuple[str, bool]]) -> dict:
+    proj = _Rel(projection_exec(exprs, r.plan), [nm for _, nm in exprs])
+    return sort_exec([(proj.c(nm), desc, False) for nm, desc in order], proj.plan)
+
+
+def _sum(name: str, e: dict, dt="Float64") -> dict:
+    return aggregate_expr("sum", name, e, dt)
+
+
+def tpch_q1(n: int = TARGET_PARTITIONS) -> dict:
+    li = _tpch_scan("lineitem", ["l_quantity", "l_extendedprice", "l_discount", "l_tax", "l_returnflag", "l_linestatus", "l_shipdate"], n)
+    li = _filter(li, lambda r: binary(r.c("l_shipdate"), "LtEq", _date("1998-09-02")))
+    disc_price = _revenue(li)
+    charge = binary(disc_price, "Multiply", binary(_f64(1), "Plus", li.c("l_tax")))
+    aggrs = [_sum("SUM(lineitem.l_quantity)", li.c("l_quantity")), _sum("SUM(lineitem.l_extendedprice)", li.c("l_extendedprice")),
+             _sum("SUM(lineitem.l_extendedprice * Int64(1) - lineitem.l_discount)", disc_price),
+             _sum("SUM(lineitem.l_extendedprice * Int64(1) - lineitem.l_discount * Int64(1) + lineitem.l_tax)", charge),
+             aggregate_expr("avg", "AVG(lineitem.l_quantity)", li.c("l_quantity"), "Float64"),
+             aggregate_expr("avg", "AVG(lineitem.l_extendedprice)", li.c("l_extendedprice"), "Float64"),
+             aggregate_expr("avg", "AVG(lineitem.l_discount)", li.c("l_discount"), "Float64"),
+             aggregate_expr("count", "COUNT(UInt8(1))", literal("UInt8", 1), "UInt64")]
+    g = _grouped(li, ["l_returnflag", "l_linestatus"], aggrs, n)
+    outs = ["sum_qty", "sum_base_price", "sum_disc_price", "sum_charge", "avg_qty", "avg_price", "avg_disc", "count_order"]
+    return _project_sort(g, [(g.c("l_returnflag"), "l_returnflag"), (g.c("l_linestatus"), "l_linestatus")] +
+                         [(g.c(a["name"]), o) for a, o in zip(aggrs, outs)], [("l_returnflag", False), ("l_linestatus", False)])
+
+
+def tpch_q3(n: int = TARGET_PARTITIONS) -> dict:
+    cu = _filter(_tpch_scan("customer", ["c_custkey", "c_mktsegment"], n), lambda r: binary(r.c("c_mktsegment"), "Eq", literal("Utf8", "BUILDING")))
+    od = _filter(_tpch_scan("orders", ["o_orderkey", "o_custkey", "o_orderdate", "o_shippriority"], n),
+                 lambda r: binary(r.c("o_orderdate"), "Lt", _date("1995-03-15")))
+    li = _filter(_tpch_scan("lineitem", ["l_orderkey", "l_extendedprice", "l_discount", "l_shipdate"], n),
+                 lambda r: binary(r.c("l_shipdate"), "Gt", _date("1995-03-15")))
+    j = _join(_join(cu, od, [("c_custkey", "o_custkey")], n), li, [("o_orderkey", "l_orderkey")], n)
+    rev = _sum("SUM(lineitem.l_extendedprice * Int64(1) - lineitem.l_discount)", _revenue(j))
+    g = _grouped(j, ["l_orderkey", "o_orderdate", "o_shippriority"], [rev], n)
+    return _project_sort(g, [(g.c("l_orderkey"), "l_orderkey"), (g.c(rev["name"]), "revenue"), (g.c("o_orderdate"), "o_orderdate"),
+                             (g.c("o_shippriority"), "o_shippriority")], [("revenue", True), ("o_orderdate", False)])
+
+
+def tpch_q5(n: int = TARGET_PARTITIONS) -> dict:
+    cu = _tpch_scan("customer", ["c_custkey", "c_nationkey"], n)
+    od = _filter(_tpch_scan("orders", ["o_orderkey", "o_custkey", "o_orderdate"], n),
+                 lambda r: _and(binary(r.c("o_orderdate"), "GtEq", _date("1994-01-01")), binary(r.c("o_orderdate"), "Lt", _date("1995-01-01"))))
+    li = _tpch_scan("lineitem", ["l_orderkey", "l_suppkey", "l_extendedprice", "l_discount"], n)
+    su = _tpch_scan("supplier", ["s_suppkey", "s_nationkey"], n)
+    na = _tpch_scan("nation", ["n_nationkey", "n_name", "n_regionkey"], n)
+    re = _filter(_tpch_scan("region", ["r_regionkey", "r_name"], n), lambda r: binary(r.c("r_name"), "Eq", literal("Utf8", "ASIA")))
+    j = _join(cu, od, [("c_custkey", "o_custkey")], n)
+    j = _join(j, li, [("o_orderkey", "l_orderkey")], n)
+    j = _join(j, su, [("l_suppkey", "s_suppkey"), ("c_nationkey", "s_nationkey")], n)
+    j = _join(j, na, [("s_nationkey", "n_nationkey")], n)
+    j = _join(j, re, [("n_regionkey", "r_regionkey")], n)
+    rev = _sum("SUM(lineitem.l_extendedprice * Int64(1) - lineitem.l_discount)", _revenue(j))
+    g = _grouped(j, ["n_name"], [rev], n)
+    return _project_sort(g, [(g.c("n_name"), "n_name"), (g.c(rev["name"]), "revenue")], [("revenue", True)])
+
+
+def tpch_q6(n: int = TARGET_PARTITIONS) -> dict:
+    li = _tpch_scan("lineitem", ["l_quantity", "l_extendedprice", "l_discount", "l_shipdate"], n)
+    # BETWEEN .06 - 0.01 AND .06 + 0.01 stays Float64 literal arithmetic: 0.06 + 0.01 = 0.06999999999999999 < 0.07
+    lo = binary(literal("Float64", 0.06), "Minus", literal("Float64", 0.01))
+    hi = binary(literal("Float64", 0.06), "Plus", literal("Float64", 0.01))
+    li = _filter(li, lambda r: _and(binary(r.c("l_shipdate"), "GtEq", _date("1994-01-01")), binary(r.c("l_shipdate"), "Lt", _date("1995-01-01")),
+                                    binary(r.c("l_discount"), "GtEq", lo), binary(r.c("l_discount"), "LtEq", hi),
+                                    binary(r.c("l_quantity"), "Lt", _f64(24))))
+    rev = _sum("SUM(lineitem.l_extendedprice * lineitem.l_discount)", binary(li.c("l_extendedprice"), "Multiply", li.c("l_discount")))
+    g = _grouped(li, [], [rev], n)
+    return projection_exec([(g.c(rev["name"]), "revenue")], g.plan)
+
+
+def tpch_q10(n: int = TARGET_PARTITIONS) -> dict:
+    cu = _tpch_scan("customer", ["c_custkey", "c_name", "c_address", "c_nationkey", "c_phone", "c_acctbal", "c_comment"], n)
+    od = _filter(_tpch_scan("orders", ["o_orderkey", "o_custkey", "o_orderdate"], n),
+                 lambda r: _and(binary(r.c("o_orderdate"), "GtEq", _date("1993-10-01")), binary(r.c("o_orderdate"), "Lt", _date("1994-01-01"))))
+    li = _filter(_tpch_scan("lineitem", ["l_orderkey", "l_extendedprice", "l_discount", "l_returnflag"], n),
+                 lambda r: binary(r.c("l_returnflag"), "Eq", literal("Utf8", "R")))
+    na = _tpch_scan("nation", ["n_nationkey", "n_name"], n)
+    j = _join(cu, od, [("c_custkey", "o_custkey")], n)
+    j = _join(j, li, [("o_orderkey", "l_orderkey")], n)
+    j = _join(j, na, [("c_nationkey", "n_nationkey")], n)
+    rev = _sum("SUM(lineitem.l_extendedprice * Int64(1) - lineitem.l_discount)", _revenue(j))
+    group = ["c_custkey", "c_name", "c_acctbal", "c_phone", "n_name", "c_address", "c_comment"]
+    g = _grouped(j, group, [rev], n)
+    return _project_sort(g, [(g.c("c_custkey"), "c_custkey"), (g.c("c_name"), "c_name"), (g.c(rev["name"]), "revenue"),
+                             (g.c("c_acctbal"), "c_acctbal"), (g.c("n_name"), "n_name"), (g.c("c_address"), "c_address"),
+                             (g.c("c_phone"), "c_phone"), (g.c("c_comment"), "c_comment")], [("revenue", True)])
+
+
+def tpch_q12(n: int = TARGET_PARTITIONS) -> dict:
+    li = _filter(_tpch_scan("lineitem", ["l_orderkey", "l_shipdate", "l_commitdate", "l_receiptdate", "l_shipmode"], n),
+                 lambda r: _and(in_list(r.c("l_shipmode"), [literal("Utf8", "MAIL"), literal("Utf8", "SHIP")]),
+                                binary(r.c("l_commitdate"), "Lt", r.c("l_receiptdate")), binary(r.c("l_shipdate"), "Lt", r.c("l_commitdate")),
+                                binary(r.c("l_receiptdate"), "GtEq", _date("1994-01-01")), binary(r.c("l_receiptdate"), "Lt", _date("1995-01-01"))))
+    od = _tpch_scan("orders", ["o_orderkey", "o_orderpriority"], n)
+    j = _join(li, od, [("l_orderkey", "o_orderkey")], n)
+    pr = j.c("o_orderpriority")
+    urgent, high = literal("Utf8", "1-URGENT"), literal("Utf8", "2-HIGH")
+    hi = case_expr([(binary(binary(pr, "Eq", urgent), "Or", binary(pr, "Eq", high)), literal("Int64", 1))], literal("Int64", 0))
+    lo = case_expr([(binary(binary(pr, "NotEq", urgent), "And", binary(pr, "NotEq", high)), literal("Int64", 1))], literal("Int64", 0))
+    aggrs = [_sum("SUM(CASE WHEN orders.o_orderpriority = Utf8(\"1-URGENT\") OR orders.o_orderpriority = Utf8(\"2-HIGH\") THEN Int64(1) ELSE Int64(0) END)", hi, "Int64"),
+             _sum("SUM(CASE WHEN orders.o_orderpriority != Utf8(\"1-URGENT\") AND orders.o_orderpriority != Utf8(\"2-HIGH\") THEN Int64(1) ELSE Int64(0) END)", lo, "Int64")]
+    g = _grouped(j, ["l_shipmode"], aggrs, n)
+    return _project_sort(g, [(g.c("l_shipmode"), "l_shipmode"), (g.c(aggrs[0]["name"]), "high_line_count"), (g.c(aggrs[1]["name"]), "low_line_count")],
+                         [("l_shipmode", False)])
+
+
+def tpch_q14(n: int = TARGET_PARTITIONS) -> dict:
+    li = _filter(_tpch_scan("lineitem", ["l_partkey", "l_extendedprice", "l_discount", "l_shipdate"], n),
+                 lambda r: _and(binary(r.c("l_shipdate"), "GtEq", _date("1995-09-01")), binary(r.c("l_shipdate"), "Lt", _date("1995-10-01"))))
+    pt = _tpch_scan("part", ["p_partkey", "p_type"], n)
+    j = _join(li, pt, [("l_partkey", "p_partkey")], n)
+    promo = case_expr([(binary(j.c("p_type"), "Like", literal("Utf8", "PROMO%")), _revenue(j))], _f64(0))
+    aggrs = [_sum("SUM(CASE WHEN part.p_type LIKE Utf8(\"PROMO%\") THEN lineitem.l_extendedprice * Int64(1) - lineitem.l_discount ELSE Int64(0) END)", promo),
+             _sum("SUM(lineitem.l_extendedprice * Int64(1) - lineitem.l_discount)", _revenue(j))]
+    g = _grouped(j, [], aggrs, n)
+    share = binary(binary(literal("Float64", 100.0), "Multiply", g.c(aggrs[0]["name"])), "Divide", g.c(aggrs[1]["name"]))
+    return projection_exec([(share, "promo_revenue")], g.plan)
+
+
+TPCH_QUERIES = {"q1": tpch_q1, "q3": tpch_q3, "q5": tpch_q5, "q6": tpch_q6, "q10": tpch_q10, "q12": tpch_q12, "q14": tpch_q14}
+# the table each MemoryExec leaf scans, in leaf (feed) order
+TPCH_SOURCES = {"q1": ["lineitem"], "q3": ["customer", "orders", "lineitem"],
+                "q5": ["customer", "orders", "lineitem", "supplier", "nation", "region"], "q6": ["lineitem"],
+                "q10": ["customer", "orders", "lineitem", "nation"], "q12": ["lineitem", "orders"], "q14": ["lineitem", "part"]}

@@ -135,7 +135,7 @@ int flockgpu_flush_l2(flockgpu_ctx* ctx);
  * `projection` (may be NULL = all columns) selects and orders the columns that are copied -- the
  * MemoryExec `projection` of the reference plan (flock/src/tests/data/plan/join.json: "projection": [0, 1]).
  * Supported column types: Int32 "i", UInt32 "I", Int64 "l", UInt64 "L", Float64 "g",
- * Timestamp "ts?:..", Utf8 "u".  Arrays with nulls are rejected with FLOCKGPU_ERR_UNSUPPORTED
+ * Timestamp "ts?:..", Date32 "tdD", Utf8 "u".  Arrays with nulls are rejected with FLOCKGPU_ERR_UNSUPPORTED
  * (every NEXMark field is non-nullable, event.rs:130-149, :220-245, :336-352).                     */
 int flockgpu_table_import(flockgpu_ctx* ctx, const struct ArrowSchema* schema,
                           const struct ArrowArray* const* batches, int32_t n_batches,
@@ -248,7 +248,8 @@ enum flockgpu_dtype {
   FLOCKGPU_FLOAT64 = 4,
   FLOCKGPU_TIMESTAMP = 5, /* int64 storage; unit/timezone carried by the Arrow format string */
   FLOCKGPU_UTF8 = 6,
-  FLOCKGPU_UINT32 = 7
+  FLOCKGPU_UINT32 = 7,
+  FLOCKGPU_DATE32 = 8     /* int32 storage: days since 1970-01-01, Arrow format "tdD" */
 };
 enum flockgpu_op {
   FLOCKGPU_OP_COLUMN = 1,   /* push column `col` of the input table                              */
@@ -274,7 +275,11 @@ enum flockgpu_op {
   /* x [NOT] IN (l1 ... ln): i64 = n (>= 1), col = 1 for NOT IN; pops, in push order, x l1 ... ln, where every l is a
    * literal token (LIT_I64 / LIT_F64 / LIT_UTF8 / LIT_NULL).  SQL's three-valued result: NULL when x is NULL, or when
    * nothing matches and a list literal is NULL.                                                                      */
-  FLOCKGPU_OP_IN_LIST = 45
+  FLOCKGPU_OP_IN_LIST = 45,
+  /* x [NOT] LIKE pattern: pops, in push order, x (Utf8) and the pattern (a LIT_UTF8, or LIT_NULL).  Case-sensitive; '%'
+   * matches any run of characters, '_' exactly one UTF-8 code point; there is no escape character.  NULL in, NULL out. */
+  FLOCKGPU_OP_LIKE = 46,
+  FLOCKGPU_OP_NOT_LIKE = 47
 };
 #define FLOCKGPU_CASE_HAS_BASE 1
 #define FLOCKGPU_CASE_HAS_ELSE 2
