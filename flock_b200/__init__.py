@@ -339,6 +339,11 @@ class Context:
     def kernel_launches(self) -> int:
         return lib.flockgpu_kernel_launches(self.handle)
 
+    @property
+    def overlapped_launches(self) -> int:
+        """Kernel launches that started while the kernel ahead of them was still running (back-to-back filters)."""
+        return lib.flockgpu_overlapped_launches(self.handle)
+
     def bytes_moved(self) -> tuple[int, int]:
         """(host -> device, device -> host) bytes this context has moved over the host link so far."""
         return lib.flockgpu_bytes_moved(self.handle, 0), lib.flockgpu_bytes_moved(self.handle, 1)

@@ -114,6 +114,7 @@ PROTOTYPES = {
     "flockgpu_timer_stop": (C.c_int, [_P, C.c_int]),
     "flockgpu_timer_elapsed_ms": (C.c_int, [_P, C.c_int, C.POINTER(C.c_float)]),
     "flockgpu_kernel_launches": (C.c_int64, [_P]),
+    "flockgpu_overlapped_launches": (C.c_int64, [_P]),
     "flockgpu_bytes_moved": (C.c_int64, [_P, C.c_int32]),
     "flockgpu_set_option": (C.c_int, [_P, C.c_char_p, C.c_int64]),
     "flockgpu_profile_begin": (C.c_int, [_P]),

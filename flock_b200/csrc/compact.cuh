@@ -362,20 +362,53 @@ __device__ __forceinline__ void cp_rank_tile(CompactSmem<E, I>& s, const Compact
 // is accepted.
 CompactScratch prepare_compact(const CtxPtr& ctx, long long num_tiles, long long resident_ctas, unsigned long long* out_count, bool rounds = false);
 
+// A launch of a kernel built to start while the kernel enqueued ahead of it drains (filter_compact_kernel<PredI32>):
+// before griddepcontrol.wait it only reads its input buffers and its own shared memory, and it touches the shared
+// scan scratch, its outputs and d_scalars only after the wait, which returns once that kernel has completed and its
+// memory is visible.
+struct EarlyStart {
+  int64_t newest_input;  // the largest Buffer::seq among the device buffers the launch reads
+  int64_t outputs;       // Buffer::seq of its outputs (ctx->alloc_seq, advanced before they were allocated)
+};
+
+// Whether this launch may take programmatic stream serialization (core.cu; the whole policy).  Only when ALL hold:
+//   - it is a single-wave (cooperative rounds) launch of an EarlyStart kernel;
+//   - the last kernel enqueued on ctx->stream was a single-wave EarlyStart launch of the same kernel (ctx->launches
+//     has advanced by that one launch since), and prepare_compact enqueued no scratch reset since;
+//   - every buffer it reads is older than that launch's outputs (Buffer::seq).  No kernel writes into a table column
+//     it did not allocate at its own enqueue: a column is written only by work its operator enqueues before it returns,
+//     and outputs are fresh blocks.  So such a buffer was complete before the previous launch started, and since that
+//     launch's CTAs pass their own wait before they let this one start, everything ahead of it has completed.  A
+//     chained input (the previous filter's output) is not older, and that launch waits as before.
+bool overlap_previous(const CtxPtr& ctx, const void* kernel, const CompactScratch& sc, const EarlyStart* early);
+// Records an accepted launch for the next overlap_previous() decision.
+void note_compact_launch(const CtxPtr& ctx, const void* kernel, const CompactScratch& sc, const EarlyStart* early, bool overlapped);
+
 // Launches a compaction kernel with sc.grid CTAs.  Single-wave launches wait for data of other CTAs, which only
 // arrives when EVERY CTA of the grid is running, so they go through the cooperative-launch path: the driver then
 // guarantees co-residency (or fails the launch) instead of us assuming the GPU is otherwise idle.
+//
+// A launch that overlaps its predecessor (overlap_previous) drops the cooperative attribute: a launch that carries both
+// is accepted but never starts before its predecessor has ended (measured on an H100 80GB HBM3, CUDA 12.9).  It
+// stays live without it: the previous grid never waits on this one, and this grid is the same kernel with the same
+// grid (resident_ctas of the same instantiation), so every one of its CTAs is resident once the previous grid exits.
 template <class Kernel, class... Args>
-inline void launch_compact(const CtxPtr& ctx, Kernel kernel, const CompactScratch& sc, Args&&... args) {
+inline void launch_compact_early(const CtxPtr& ctx, Kernel kernel, const CompactScratch& sc, const EarlyStart* early, Args&&... args) {
   HostSpan span("launch_compact");
+  const bool overlap = overlap_previous(ctx, reinterpret_cast<const void*>(kernel), sc, early);
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(unsigned(sc.grid));
   cfg.blockDim = dim3(CP_THREADS);
   cfg.dynamicSmemBytes = 0;
   cfg.stream = ctx->stream;
   cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeCooperative;
-  attr[0].val.cooperative = sc.single_wave ? 1 : 0;
+  if (overlap) {
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+  } else {
+    attr[0].id = cudaLaunchAttributeCooperative;
+    attr[0].val.cooperative = sc.single_wave ? 1 : 0;
+  }
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   FG_CUDA(cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...));
@@ -384,6 +417,12 @@ inline void launch_compact(const CtxPtr& ctx, Kernel kernel, const CompactScratc
   ScanScratch& s = ctx->scan;
   if (sc.single_wave) s.arrived += unsigned(sc.num_tiles);                      // one arrival per tile, no tickets
   else s.tickets_issued += unsigned(sc.num_tiles) + unsigned(sc.grid);          // every CTA draws exactly one ticket past the end
+  note_compact_launch(ctx, reinterpret_cast<const void*>(kernel), sc, early, overlap);
+}
+
+template <class Kernel, class... Args>
+inline void launch_compact(const CtxPtr& ctx, Kernel kernel, const CompactScratch& sc, Args&&... args) {
+  launch_compact_early(ctx, kernel, sc, static_cast<const EarlyStart*>(nullptr), std::forward<Args>(args)...);
 }
 
 // Rank of survivor item k among the survivors of its tile (0 .. tile_total - 1) / its global output position.

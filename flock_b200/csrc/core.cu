@@ -240,7 +240,7 @@ void CtxCore::drop_cached_blocks() {
   cudaStreamSynchronize(stream);
 }
 
-Buffer::Buffer(CtxPtr c, size_t n) : ctx(std::move(c)), bytes(n) {
+Buffer::Buffer(CtxPtr c, size_t n) : ctx(std::move(c)), bytes(n), seq(ctx->alloc_seq) {
   HostSpan span("alloc");
   size_t want = n ? n : 16;
   want = (want + 255) & ~size_t(255);  // room for vector tails: kernels may read up to 16 B past the end
@@ -290,6 +290,7 @@ CompactScratch prepare_compact(const CtxPtr& ctx, long long num_tiles, long long
     FG_CUDA(cudaMemsetAsync(s.ep_state, 0, size_t(cap) * stride * sizeof(unsigned long long), ctx->stream));
     FG_CUDA(cudaMemsetAsync(s.ep_counts, 0, size_t(cap) * sizeof(unsigned long long), ctx->stream));
     s.ep_capacity = cap;
+    ctx->overlap_kernel = nullptr;  // the next launch must not start before these memsets
   }
   s.epoch = (s.epoch + 1) & 0xfffffu;
   if (s.epoch == 0) {
@@ -297,6 +298,7 @@ CompactScratch prepare_compact(const CtxPtr& ctx, long long num_tiles, long long
     FG_CUDA(cudaMemsetAsync(s.ep_state, 0, size_t(s.ep_capacity) * stride * sizeof(unsigned long long), ctx->stream));
     FG_CUDA(cudaMemsetAsync(s.ep_counts, 0, size_t(s.ep_capacity) * sizeof(unsigned long long), ctx->stream));
     s.epoch = 1;
+    ctx->overlap_kernel = nullptr;
   }
   CompactScratch sc{};
   sc.tile_state = s.ep_state;
@@ -316,6 +318,18 @@ CompactScratch prepare_compact(const CtxPtr& ctx, long long num_tiles, long long
   sc.poll_sleep_ns = scan_poll_sleep_ns();
   // the arrival / ticket bases advance in launch_compact(), after the launch has been accepted
   return sc;
+}
+
+bool overlap_previous(const CtxPtr& ctx, const void* kernel, const CompactScratch& sc, const EarlyStart* early) {
+  return early && sc.single_wave && kernel == ctx->overlap_kernel && ctx->launches.load(std::memory_order_relaxed) == ctx->overlap_launches + 1 &&
+         early->newest_input < ctx->overlap_outputs;
+}
+
+void note_compact_launch(const CtxPtr& ctx, const void* kernel, const CompactScratch& sc, const EarlyStart* early, bool overlapped) {
+  ctx->overlap_kernel = early && sc.single_wave ? kernel : nullptr;
+  ctx->overlap_launches = ctx->launches.load(std::memory_order_relaxed);
+  ctx->overlap_outputs = early ? early->outputs : 0;
+  if (overlapped) ctx->overlapped.fetch_add(1, std::memory_order_relaxed);
 }
 
 int resident_ctas(const CtxPtr& ctx, const void* kernel, int threads, size_t smem) {
@@ -347,6 +361,7 @@ void read_scalars(const CtxPtr& ctx, int first, int n, unsigned long long* out) 
                           cudaMemcpyDeviceToHost, ctx->stream));
   FG_CUDA(cudaStreamSynchronize(ctx->stream));
   for (int i = 0; i < n; ++i) out[i] = ctx->h_scalars[first + i];
+  dump_filter_traces(ctx);
 }
 
 // ---- row counts in flight ------------------------------------------------------------------------
@@ -357,6 +372,7 @@ int64_t PendingRows::wait() {
     FG_CUDA(cudaEventSynchronize(ev));
     value = int64_t(ctx->h_scalars[CtxCore::kScalars + slot]);
     done = true;
+    dump_filter_traces(ctx);
     if (h2d_bytes_per_row) ctx->h2d_bytes.fetch_add(value * h2d_bytes_per_row, std::memory_order_relaxed);
   }
   return value;
@@ -1269,6 +1285,7 @@ int flockgpu_close(flockgpu_ctx* ctx) {
     if (ctx->core && ctx->core->stream) {
       cudaSetDevice(ctx->core->device);
       cudaStreamSynchronize(ctx->core->stream);
+      dump_filter_traces(ctx->core);
     }
     delete ctx;
     host_trace_dump(false);
@@ -1279,6 +1296,7 @@ int flockgpu_synchronize(flockgpu_ctx* ctx) {
   return guarded([&] {
     auto c = core_of(ctx);
     FG_CUDA(cudaStreamSynchronize(c->stream));
+    dump_filter_traces(c);
   });
 }
 
@@ -1308,6 +1326,8 @@ int flockgpu_timer_elapsed_ms(flockgpu_ctx* ctx, int slot, float* ms) {
 }
 
 int64_t flockgpu_kernel_launches(flockgpu_ctx* ctx) { return ctx && ctx->core ? ctx->core->launches.load() : -1; }
+
+int64_t flockgpu_overlapped_launches(flockgpu_ctx* ctx) { return ctx && ctx->core ? ctx->core->overlapped.load() : -1; }
 
 int64_t flockgpu_bytes_moved(flockgpu_ctx* ctx, int32_t direction) {
   if (!ctx || !ctx->core) return -1;

@@ -353,6 +353,7 @@ __global__ void __launch_bounds__(FP_THREADS, COMPUTED && PredFn::MIN_CTAS > 2 ?
     if (a.trace && tid == 0) {
       unsigned smid;
       asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
+      a.trace[tile * FP_TRACE_WORDS + 5] = 0;  // the CTA's last tile stamps its end afterwards
       a.trace[tile * FP_TRACE_WORDS + 6] = blockIdx.x;
       a.trace[tile * FP_TRACE_WORDS + 7] = smid;
     }
@@ -365,6 +366,14 @@ __global__ void __launch_bounds__(FP_THREADS, COMPUTED && PredFn::MIN_CTAS > 2 ?
     // the offset of tile r - 1 and writes its survivors.  So the loads stream while the CTA ranks, waits and writes,
     // and a round's counts are published without waiting for anybody's writes.  Tile indices are 32-bit here (2^31
     // tiles are far beyond any relation): 64-bit loop state would not fit the 64-register budget of four CTAs per SM.
+    //
+    // A launch may start while the filter launched ahead of it drains (compact.cuh: EarlyStart, launch_compact_early).
+    // Until griddepcontrol.wait, right before its first publish, a CTA only streams its first tiles into shared memory,
+    // tests and ranks the first one and prefetches its survivors: nothing there touches the scan scratch (the previous
+    // launch may still poll those words), the outputs (their blocks may have been released while it ran) or
+    // d_scalars.  Past the wait the previous launch has completed and its memory is visible.  The CTA lets the next
+    // launch start (launch_dependents) once it has passed its wait and issued its last tile's loads, so at most one
+    // launch runs ahead of the current one.  Without the launch attribute both instructions do nothing.
     __shared__ CompactSmem<E, I> rank_sm[2];  // tile r is ranked into rank_sm[r & 1] and written from it one iteration later
     __shared__ unsigned long long rounds_done;
     const int num_tiles = int(sc.num_tiles);
@@ -389,7 +398,10 @@ __global__ void __launch_bounds__(FP_THREADS, COMPUTED && PredFn::MIN_CTAS > 2 ?
         for (int g = 0; g < G; ++g) packed[g >> 2] |= lane_prefix[g] << ((g & 3) * 8);
         stamp(tile, 2);
         prefetch_survivors<E>(a, bits, int64_t(tile) * TILE, tid);
+        if (it == 0) asm volatile("griddepcontrol.wait;" ::: "memory");
         cp_round_publish(sc, tile, rank_sm[it & 1].tile_total);
+        // the first iteration with no loads left to issue (tile + grid, if any, was issued above)
+        if (tile + 2 * sc.grid >= num_tiles && (it == 0 || tile + sc.grid < num_tiles)) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
       }
       if (it > 0) {
         CompactSmem<E, I>& ps = rank_sm[(it - 1) & 1];
@@ -527,42 +539,54 @@ void fill_colrefs(const Table& t, ColRef* refs) {
 // of the instantiation launched: functors with ROUNDS walk any number of cooperative rounds; the others run one
 // wave when the tiles fit it and fall back to decoupled look-back beyond it.
 template <class PredFn, bool COMPUTED>
-static void launch_filter(const CtxPtr& ctx, const PredFn& pred, FilterArgs args, const char* profile_name = "filter_compact_kernel") {
+static void launch_filter(const CtxPtr& ctx, const PredFn& pred, FilterArgs args, const char* profile_name = "filter_compact_kernel",
+                          const EarlyStart* early = nullptr) {
   constexpr int64_t TILE = int64_t(FP_THREADS) * PredFn::I;
   const int64_t num_tiles = (args.n_rows + TILE - 1) / TILE;
   auto* kernel = &filter_compact_kernel<PredFn, COMPUTED>;
   args.sc = prepare_compact(ctx, num_tiles, resident_ctas(ctx, reinterpret_cast<const void*>(kernel), FP_THREADS), args.out_count, PredFn::ROUNDS);
-  const int grid = args.sc.grid;
   args.sc.host_count = args.host_count;
   BufferPtr trace_buf;
   static const char* trace_path = getenv("FLOCKGPU_TRACE");
-  const size_t trace_words = size_t(num_tiles) * FP_TRACE_WORDS;
   if (trace_path) {
-    trace_buf = alloc(ctx, trace_words * 8);
-    FG_CUDA(cudaMemsetAsync(trace_buf->ptr, 0, trace_words * 8, ctx->stream));
+    // every word of every tile is stamped by the kernel: no memset, which would stand between two launches
+    trace_buf = alloc(ctx, size_t(num_tiles) * FP_TRACE_WORDS * 8);
     args.trace = trace_buf->as<unsigned long long>();
   }
+  const int64_t overlapped0 = ctx->overlapped.load(std::memory_order_relaxed);
   {
     LaunchTimer lt(ctx, profile_name);
-    launch_compact(ctx, kernel, args.sc, pred, args);
+    // only the rounds path waits for the previous grid before it touches shared state
+    launch_compact_early(ctx, kernel, args.sc, PredFn::ROUNDS ? early : nullptr, pred, args);
   }
   FG_CUDA(cudaGetLastError());
   count_launch(ctx);
-  if (trace_path) {
-    // debug only: dump the per-tile time stamps of this launch (overwrites the file each launch).  Header: tiles, grid,
-    // 1 when tile t ran in round t / grid of the cooperative mode (0: decoupled look-back).
-    std::vector<unsigned long long> h(trace_words);
-    FG_CUDA(cudaMemcpyAsync(h.data(), trace_buf->ptr, h.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    FG_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (FILE* f = fopen(trace_path, "w")) {
-      fprintf(f, "%lld %d %d\n", (long long)num_tiles, grid, args.sc.single_wave);
-      for (size_t i = 0; i < h.size() / FP_TRACE_WORDS; ++i) {
-        for (int j = 0; j < FP_TRACE_WORDS; ++j) fprintf(f, "%llu ", h[i * FP_TRACE_WORDS + j]);
-        fprintf(f, "\n");
-      }
-      fclose(f);
+  if (trace_path)
+    ctx->filter_traces.push_back({trace_buf, (long long)num_tiles, args.sc.grid, args.sc.single_wave,
+                                  int(ctx->overlapped.load(std::memory_order_relaxed) != overlapped0)});
+}
+
+void dump_filter_traces(const CtxPtr& ctx) {
+  static const char* trace_path = getenv("FLOCKGPU_TRACE");
+  if (!trace_path || ctx->filter_traces.empty()) return;
+  // debug only: the per-tile time stamps of the launches since the last dump, in launch order (overwrites the file).
+  // Per launch a header: tiles, grid, 1 when tile t ran in round t / grid of the cooperative mode (0: decoupled
+  // look-back), 1 when the launch was allowed to overlap the one before it; then one line of stamps per tile.
+  std::vector<CtxCore::FilterTrace> traces;
+  traces.swap(ctx->filter_traces);
+  FG_CUDA(cudaStreamSynchronize(ctx->stream));
+  FILE* f = fopen(trace_path, "w");
+  if (!f) return;
+  for (const CtxCore::FilterTrace& t : traces) {
+    std::vector<unsigned long long> h(size_t(t.tiles) * FP_TRACE_WORDS);
+    FG_CUDA(cudaMemcpy(h.data(), t.stamps->ptr, h.size() * 8, cudaMemcpyDeviceToHost));
+    fprintf(f, "%lld %d %d %d\n", t.tiles, t.grid, t.rounds, t.overlapped);
+    for (size_t i = 0; i < h.size() / FP_TRACE_WORDS; ++i) {
+      for (int j = 0; j < FP_TRACE_WORDS; ++j) fprintf(f, "%llu ", h[i * FP_TRACE_WORDS + j]);
+      fprintf(f, "\n");
     }
   }
+  fclose(f);
 }
 
 TablePtr filter_project(const CtxPtr& ctx, const TablePtr& in_ptr, const Expr* predicate, const std::vector<Expr>& projections,
@@ -816,6 +840,15 @@ TablePtr filter_project(const CtxPtr& ctx, const TablePtr& in_ptr, const Expr* p
   fa.out_count = ctx->d_scalars + 0;
   fa.err_flag = err_flag;
   fill_colrefs(in, fa.cols);
+  // What a launch that starts before the kernel ahead of it completes reads early (compact.cuh: EarlyStart): the
+  // relation's device-resident buffers, all older than the outputs allocated below.
+  EarlyStart early{0, ++ctx->alloc_seq};
+  bool may_start_early = true;
+  for (const Column& c : in.cols) {
+    may_start_early &= !c.chunks;
+    for (const BufferPtr& b : {c.data, c.offsets, c.validity})
+      if (b) early.newest_input = std::max(early.newest_input, b->seq);
+  }
 
   bool need_sel = false;
   std::vector<int> utf8_outs;
@@ -883,8 +916,9 @@ TablePtr filter_project(const CtxPtr& ctx, const TablePtr& in_ptr, const Expr* p
   for (int c = 0; c < fa.n_out; ++c) computed |= fa.outs[c].kind != OUT_PASS;
   auto launch = [&](const auto& pred) {
     using PredFn = std::decay_t<decltype(pred)>;
-    if (computed) launch_filter<PredFn, true>(ctx, pred, fa);
-    else launch_filter<PredFn, false>(ctx, pred, fa);
+    const EarlyStart* e = may_start_early && !check_err ? &early : nullptr;  // check_err: a memset goes first
+    if (computed) launch_filter<PredFn, true>(ctx, pred, fa, "filter_compact_kernel", e);
+    else launch_filter<PredFn, false>(ctx, pred, fa, "filter_compact_kernel", e);
   };
   auto launch_i32 = [&](int64_t modulus) {
     const Column& pc = in.cols[cp.fast.col];

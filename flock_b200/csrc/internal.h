@@ -133,6 +133,21 @@ struct CtxCore {
   cudaEvent_t timer_start[16] = {};
   cudaEvent_t timer_stop[16] = {};
   std::atomic<int64_t> launches{0};
+  // Back-to-back PredI32 filter launches overlap (programmatic dependent launch, compact.cuh: launch_compact_early).
+  // overlap_kernel: the kernel of the last launch that its successor may overlap (nullptr: none), with `launches`
+  // just before it was enqueued and the Buffer::seq of its outputs.
+  const void* overlap_kernel = nullptr;
+  int64_t overlap_launches = 0, overlap_outputs = 0;
+  int64_t alloc_seq = 0;               // Buffer::seq of new buffers; a filter advances it before it allocates its outputs
+  std::atomic<int64_t> overlapped{0};  // launches that took the attribute (flockgpu_overlapped_launches)
+  // FLOCKGPU_TRACE: per-tile stamp buffers of the filter launches enqueued since the stream last synchronised
+  // (filter_project.cu), written to the trace file at the next synchronising call so that launches may overlap
+  struct FilterTrace {
+    std::shared_ptr<struct Buffer> stamps;
+    long long tiles;
+    int grid, rounds, overlapped;
+  };
+  std::vector<FilterTrace> filter_traces;
   // bytes that crossed the host link on behalf of this context (flockgpu_bytes_moved): copies issued by import /
   // export plus what kernels read in place from page-locked batches (zero-copy feed)
   std::atomic<int64_t> h2d_bytes{0}, d2h_bytes{0};
@@ -235,11 +250,15 @@ struct Buffer {
   void* ptr = nullptr;
   size_t bytes = 0;
   size_t block_bytes = 0;  // size class of an owned block (CtxCore::take_block)
+  // ctx->alloc_seq when the buffer was allocated (a view: when its owner was): a launch may read the buffer before the
+  // kernel enqueued ahead of it completes only when the buffer is older than that kernel's outputs (compact.cuh)
+  int64_t seq = 0;
   // A VIEW (a slice of another allocation: one partition of a partition-ordered relation, a column inside a
   // peer-exchange window) keeps its owner alive through `parent` and frees nothing itself.
   std::shared_ptr<const void> parent;
   Buffer(CtxPtr c, size_t n);
-  Buffer(CtxPtr c, void* p, size_t n, std::shared_ptr<const void> owner) : ctx(std::move(c)), ptr(p), bytes(n), parent(std::move(owner)) {}
+  Buffer(CtxPtr c, void* p, size_t n, std::shared_ptr<const void> owner)
+      : ctx(std::move(c)), ptr(p), bytes(n), seq(ctx->alloc_seq), parent(std::move(owner)) {}
   ~Buffer();
   Buffer(const Buffer&) = delete;
   Buffer& operator=(const Buffer&) = delete;
@@ -252,7 +271,9 @@ using BufferPtr = std::shared_ptr<Buffer>;
 BufferPtr alloc(const CtxPtr& ctx, size_t bytes);  // bytes == 0 still yields a valid (tiny) buffer
 // `bytes` bytes of `b` starting at byte `off`; the caller keeps `off` 16-byte aligned when vector loads will read it
 inline BufferPtr view_of(const BufferPtr& b, size_t off, size_t bytes) {
-  return std::make_shared<Buffer>(b->ctx, static_cast<char*>(b->ptr) + off, bytes, std::static_pointer_cast<const void>(b));
+  auto v = std::make_shared<Buffer>(b->ctx, static_cast<char*>(b->ptr) + off, bytes, std::static_pointer_cast<const void>(b));
+  v->seq = b->seq;
+  return v;
 }
 
 // Grid-prefix tuning (FLOCKGPU_LB_STRIDE / FLOCKGPU_LB_SLEEP override): 64-bit words between the look-back words of
@@ -267,6 +288,9 @@ int resident_ctas(const CtxPtr& ctx, const void* kernel, int threads, size_t sme
 void stage_copy(void* dst, const void* src, size_t n, int streaming);
 // Copies `n` u64 scalars from d_scalars[first..] to the host and waits.
 void read_scalars(const CtxPtr& ctx, int first, int n, unsigned long long* out);
+// FLOCKGPU_TRACE: writes the stamps of the filter launches enqueued since the last call to the trace file
+// (filter_project.cu); called where the stream synchronises anyway.  No-op when there are none.
+void dump_filter_traces(const CtxPtr& ctx);
 
 // ------------------------------------------------------------------------------------------------
 // columns and tables

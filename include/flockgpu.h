@@ -94,6 +94,9 @@ int flockgpu_timer_stop(flockgpu_ctx* ctx, int slot);              /* records th
 int flockgpu_timer_elapsed_ms(flockgpu_ctx* ctx, int slot, float* ms); /* syncs on the stop event  */
 /* Number of kernels this library has launched on the ctx since it was opened.                     */
 int64_t flockgpu_kernel_launches(flockgpu_ctx* ctx);
+/* How many of those launches were allowed to start while the kernel ahead of them on the stream was still running
+ * (programmatic dependent launch: back-to-back integer-predicate filters over independent relations).             */
+int64_t flockgpu_overlapped_launches(flockgpu_ctx* ctx);
 /* Bytes that have crossed the host link for this ctx since it was opened: direction 0 = host -> device (copies issued
  * by table import / feed_data_sources plus what kernels read in place from page-locked batches under "feed_zero_copy"),
  * 1 = device -> host (table export).  bench.py's e2e leg reports the difference across its timed region.             */
