@@ -193,6 +193,7 @@ TablePtr dim_count_aggregate(const CtxPtr& ctx, const TablePtr& fact_ptr, int fa
       for (const Column& c : fact.cols) infos.push_back({c.dtype, c.name, c.format, c.validity != nullptr});
       CompiledPredicate cp = compile_predicate(*predicate, infos);
       FG_CHECK(!cp.prog.has_div_by_col, FLOCKGPU_ERR_INVALID, "dim_count: a predicate that divides by a column stays in its own filter");
+      FG_CHECK(!cp.lossy_cast, FLOCKGPU_ERR_INVALID, "dim_count: a predicate with a CAST that can give NULL stays in its own filter");
       a.has_pred = 1;
       a.pred = cp.prog;
     }

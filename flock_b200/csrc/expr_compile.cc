@@ -57,6 +57,17 @@ int promote(int a, int b) {
   return rank(a) >= rank(b) ? a : b;
 }
 
+// A CAST from `from` to `to` that some source value does not survive (cast_fits): Float64 to an integer type, an
+// integer type to a narrower one or across signedness.  The tree form gives NULL for the values that do not fit.  The
+// chain form has no NULLs of its own: it lowers an explicit one as a plain conversion and flags it (`lossy_cast` of
+// CompiledValue / CompiledPredicate), and the operators evaluate a flagged expression in the tree form.
+bool lossy_cast(int from, int to) {
+  if (from == to || to == FLOCKGPU_FLOAT64) return false;
+  if (from == FLOCKGPU_FLOAT64) return true;
+  if (to == FLOCKGPU_INT32 || to == FLOCKGPU_UINT32) return true;
+  return to == FLOCKGPU_UINT64 ? !is_unsigned(from) : from == FLOCKGPU_UINT64;
+}
+
 struct Tree {
   std::vector<Node> nodes;
   int root = -1;
@@ -232,6 +243,7 @@ Val literal_as(const Node& n, int dtype) {
 struct ChainBuilder {
   const Tree& t;
   bool div_by_col = false;
+  bool lossy = false;  // an explicit CAST that can lose its value, lowered without its NULLs
   explicit ChainBuilder(const Tree& tree) : t(tree) {}
 
   static void push(Chain& c, ChainStep st) {
@@ -250,7 +262,7 @@ struct ChainBuilder {
     if (to == FLOCKGPU_FLOAT64) {
       push_unary(c, is_unsigned(from) ? C_U2F : C_I2F);
     } else if (from == FLOCKGPU_FLOAT64) {
-      push_unary(c, C_F2I);
+      push_unary(c, to == FLOCKGPU_UINT64 ? C_F2U : C_F2I);
       if (to == FLOCKGPU_INT32) push_unary(c, C_WRAP_I32);
       if (to == FLOCKGPU_UINT32) push_unary(c, C_WRAP_U32);
     } else {
@@ -267,10 +279,8 @@ struct ChainBuilder {
     int src_dtype = n->dtype;
     while (n->op == FLOCKGPU_OP_CAST) {
       const Node* inner = &t.nodes[n->l];
-      // only widening / to-float casts keep the operand simple
-      bool widening = (n->dtype == FLOCKGPU_FLOAT64) || (is_intlike(n->dtype) && is_intlike(inner->dtype) && dtype_width(n->dtype) >= dtype_width(inner->dtype));
-      if (!widening && !is_literal(*inner)) return false;
-      if (inner->dtype == FLOCKGPU_FLOAT64 && n->dtype != FLOCKGPU_FLOAT64 && !is_literal(*inner)) return false;
+      // only casts that keep every value (widening, to Float64) keep the operand simple
+      if (lossy_cast(inner->dtype, n->dtype)) return false;
       src_dtype = n->dtype;
       n = inner;
     }
@@ -347,6 +357,7 @@ struct ChainBuilder {
       return c;
     }
     if (n.op == FLOCKGPU_OP_CAST) {
+      lossy |= lossy_cast(t.nodes[n.l].dtype, n.dtype);
       c = build(n.l);
       convert(c, t.nodes[n.l].dtype, n.dtype);
       return c;
@@ -449,6 +460,7 @@ CompiledValue compile_value(const Expr& e, const std::vector<ColInfo>& cols) {
   ChainBuilder b(t);
   out.chain = b.build(t.root);
   out.has_div_by_col = b.div_by_col;
+  out.lossy_cast = b.lossy;
   out.format = default_format(root.dtype);
   if (root.dtype == FLOCKGPU_TIMESTAMP) {
     // keep the unit/timezone of the first timestamp column the expression touches
@@ -545,6 +557,7 @@ CompiledPredicate compile_predicate(const Expr& e, const std::vector<ColInfo>& c
   };
   collect(t.root);
   p.has_div_by_col = b.div_by_col ? 1 : 0;
+  out.lossy_cast = b.lossy;
   bool any_null = false;
   for (int i = 0; i < p.n_terms; ++i) any_null |= p.terms[i].null_cols != 0;
 
@@ -703,6 +716,18 @@ struct TreeBuilder {
     if (to == FLOCKGPU_UINT32) return unary(T_ARITH, C_WRAP_U32, id);
     return id;
   }
+  // An explicit CAST.  One that can lose its value checks the source (cast_fits) and is NULL where it does not fit;
+  // a value that fits keeps its canonical form, except that a float is truncated toward zero.
+  int cast(int id, int from, int to) {
+    if (!lossy_cast(from, to)) return convert(id, from, to);
+    TNode n;
+    n.op = T_ARITH;
+    n.sub = from != FLOCKGPU_FLOAT64 ? C_NOP : to == FLOCKGPU_UINT64 ? C_F2U : C_F2I;
+    n.a = id;
+    n.lit.i = cast_code(from == FLOCKGPU_FLOAT64 ? DOM_F64 : is_unsigned(from) ? DOM_U64 : DOM_I64, to);
+    n.may_null = true;
+    return intern(n);
+  }
   int pooled(const std::string& s, Val* where) {
     size_t at = pool.find(s);
     if (at == std::string::npos || s.empty()) {
@@ -775,7 +800,7 @@ struct TreeBuilder {
         fail(FLOCKGPU_ERR_UNSUPPORTED, "expression: a Utf8 literal is only supported as a comparison operand or in an IN list");
       case FLOCKGPU_OP_CAST:
         FG_CHECK(t.nodes[n.l].dtype != FLOCKGPU_BOOL, FLOCKGPU_ERR_UNSUPPORTED, "expression: CAST of a boolean");
-        id = convert(lower(t, n.l, memo), t.nodes[n.l].dtype, n.dtype);
+        id = cast(lower(t, n.l, memo), t.nodes[n.l].dtype, n.dtype);
         break;
       case FLOCKGPU_OP_NEG:
         if (n.dtype == FLOCKGPU_FLOAT64) {

@@ -35,6 +35,7 @@ struct FastPred {
 struct CompiledPredicate {
   Predicate prog;
   FastPred fast;
+  bool lossy_cast = false;  // holds a CAST that can give NULL, lowered without it: the operators take the tree form
 };
 
 enum FastValueKind {
@@ -48,6 +49,7 @@ struct CompiledValue {
   int dtype = FLOCKGPU_INT64;
   std::string format;  // Arrow format of the result
   bool has_div_by_col = false;
+  bool lossy_cast = false;  // holds a CAST that can give NULL, lowered without it: the operators take the tree form
   int fast = FAST_VAL_NONE;
   double fast_lit = 0;
 };

@@ -32,7 +32,7 @@ enum ChainOp : int16_t {
   C_ADD_I, C_SUB_I, C_RSUB_I, C_MUL_I, C_DIV_I, C_RDIV_I, C_MOD_I, C_RMOD_I,
   C_DIV_U, C_RDIV_U, C_MOD_U, C_RMOD_U,
   C_ADD_F, C_SUB_F, C_RSUB_F, C_MUL_F, C_DIV_F, C_RDIV_F,
-  C_I2F, C_U2F, C_F2I, C_WRAP_I32, C_WRAP_U32
+  C_I2F, C_U2F, C_F2I, C_WRAP_I32, C_WRAP_U32, C_F2U
 };
 
 enum Cvt : int8_t { CVT_NONE = 0, CVT_I2F = 1, CVT_U2F = 2 };
@@ -113,14 +113,22 @@ struct OutCol {
 #define FG_I2F(a) __ll2double_rn(a)
 #define FG_U2F(a) __ull2double_rn(a)
 #define FG_F2I(a) __double2ll_rz(a)
+#define FG_F2U(a) __double2ull_rz(a)
 #else  // host build of the same interpreter (flockgpu_selftest_* only; never on the product path)
+// Float -> integer conversions only run on values that fit (cast_fits); the host forms still clamp, so that no input
+// is undefined behaviour.
+inline int64_t host_f2i(double d) {
+  return d != d ? 0 : d >= 9223372036854775808.0 ? INT64_MAX : d < -9223372036854775808.0 ? INT64_MIN : static_cast<int64_t>(d);
+}
+inline uint64_t host_f2u(double d) { return !(d > -1.0) ? 0 : d >= 18446744073709551616.0 ? UINT64_MAX : static_cast<uint64_t>(d); }
 #define FG_DADD(a, b) ((a) + (b))
 #define FG_DSUB(a, b) ((a) - (b))
 #define FG_DMUL(a, b) ((a) * (b))
 #define FG_DDIV(a, b) ((a) / (b))
 #define FG_I2F(a) static_cast<double>(a)
 #define FG_U2F(a) static_cast<double>(a)
-#define FG_F2I(a) static_cast<int64_t>(a)
+#define FG_F2I(a) host_f2i(a)
+#define FG_F2U(a) host_f2u(a)
 #endif
 
 FG_HD Val load_val(const ColRef& c, int64_t row) {
@@ -166,11 +174,34 @@ FG_HD Val apply_step(int op, Val a, Val b, int* err) {
     case C_I2F: r.d = FG_I2F(a.i); break;
     case C_U2F: r.d = FG_U2F(a.u); break;
     case C_F2I: r.i = FG_F2I(a.d); break;
+    case C_F2U: r.u = FG_F2U(a.d); break;
     case C_WRAP_I32: r.i = int64_t(int32_t(uint32_t(a.u))); break;
     case C_WRAP_U32: r.u = uint64_t(uint32_t(a.u)); break;
     default: break;
   }
   return r;
+}
+
+// An explicit CAST that can lose its value (Float64 to an integer type, an integer type to a narrower one or across
+// signedness) yields NULL where the target type cannot hold the source value, as arrow-rs's numeric cast does
+// (num::cast::cast returns None: NaN, +-inf, a float outside the range once truncated toward zero, an integer outside
+// the range).  code = cast_code(domain of the source, target dtype); `v` is in the canonical form of the source.
+FG_HD int64_t cast_code(int dom, int to) { return (int64_t(to) << 2) | dom; }
+
+FG_HD bool cast_fits(int64_t code, Val v) {
+  const int dom = int(code & 3), to = int(code >> 2);
+  const bool wide = to != FLOCKGPU_INT32 && to != FLOCKGPU_UINT32 && to != FLOCKGPU_DATE32;
+  const bool uns = to == FLOCKGPU_UINT32 || to == FLOCKGPU_UINT64;
+  if (dom == DOM_F64) {
+    // truncation toward zero keeps the open interval (min - 1, max + 1); every bound below is an exact double, and
+    // -9223372036854777856 is the next double below -2^63
+    const double below = uns ? -1.0 : wide ? -9223372036854777856.0 : -2147483649.0;
+    const double above = wide ? (uns ? 18446744073709551616.0 : 9223372036854775808.0) : (uns ? 4294967296.0 : 2147483648.0);
+    return v.d > below && v.d < above;  // false for NaN
+  }
+  if (dom == DOM_U64) return v.u <= (wide ? (uns ? UINT64_MAX : uint64_t(INT64_MAX)) : (uns ? uint64_t(UINT32_MAX) : uint64_t(INT32_MAX)));
+  if (uns) return v.i >= 0 && (wide || v.i <= int64_t(UINT32_MAX));
+  return wide || (v.i >= INT32_MIN && v.i <= INT32_MAX);
 }
 
 // Evaluates `c` for R rows at once: row[j] (j < R); rows < 0 are skipped.  The switch on the step

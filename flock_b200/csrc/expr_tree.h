@@ -30,7 +30,8 @@ constexpr int TREE_POOL_BYTES = 512;
 enum TreeOp : int16_t {
   T_COL = 1,      // r[d] = column `col` (a Utf8 column loads its NULL flag only)
   T_LIT,          // r[d] = lit; a != 0: a NULL literal
-  T_ARITH,        // r[d] = apply_step(sub, r[a], r[b]); b < 0: unary (conversions, wraps)
+  T_ARITH,        // r[d] = apply_step(sub, r[a], r[b]); b < 0: unary (conversions, wraps); lit != 0: an explicit CAST
+                  // that can lose its value, lit = its cast_code: NULL where !cast_fits
   T_CMP,          // r[d] = r[a] CMP r[b]; sub = domain << 8 | (cmp - FLOCKGPU_OP_EQ)
   T_CMP_UTF8,     // r[d] = column `col` CMP (column `col2` | pooled literal lit = offset << 32 | length); sub = cmp
   T_AND, T_OR,    // Kleene
@@ -176,7 +177,9 @@ FG_HD unsigned eval_tree(const TreeProgram& p, const ColRef* cols, const TreeOut
           Val v;
           v.i = 0;
           uint8_t nf = f;
-          if (!(f & TF_NULL)) {
+          if (!(f & TF_NULL) && in.lit.i && !cast_fits(in.lit.i, rf.val(in.a, j))) {
+            nf |= TF_NULL;
+          } else if (!(f & TF_NULL)) {
             int e = 0;
             v = apply_step(in.sub, rf.val(in.a, j), in.b >= 0 ? rf.val(in.b, j) : v, &e);
             if (e) nf |= TF_ERR;

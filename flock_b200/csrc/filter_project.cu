@@ -641,6 +641,9 @@ TablePtr filter_project(const CtxPtr& ctx, const TablePtr& in_ptr, const Expr* p
         for (int st = 0; st < v.chain.n_steps; ++st)
           if (v.chain.steps[st].src == 1) note(v.chain.steps[st].col);
         if (!v.passthrough && null_inputs > (predicate ? 0 : 4)) fail(FLOCKGPU_ERR_UNSUPPORTED, "projection: more NULL inputs than the chain form carries");
+        // a NULL operand makes the quotient NULL, whatever value sits under it: the chain form divides it all the same
+        if (v.has_div_by_col && null_inputs > 0) fail(FLOCKGPU_ERR_UNSUPPORTED, "projection: a division over columns with NULLs");
+        if (v.lossy_cast) fail(FLOCKGPU_ERR_UNSUPPORTED, "projection: a CAST that can give NULL");
         vals.push_back(v);
         tree_vals.push_back(false);
       } catch (const Error& err) {
@@ -801,6 +804,9 @@ TablePtr filter_project(const CtxPtr& ctx, const TablePtr& in_ptr, const Expr* p
   bool use_tree = false;
   try {
     cp = compile_predicate(*predicate, infos);
+    // the term form divides in the rows where an operand is NULL too (kleene: a referenced column has NULLs)
+    if (cp.prog.has_div_by_col && cp.prog.kleene) fail(FLOCKGPU_ERR_UNSUPPORTED, "filter: a division over columns with NULLs");
+    if (cp.lossy_cast) fail(FLOCKGPU_ERR_UNSUPPORTED, "filter: a CAST that can give NULL");
   } catch (const Error& err) {
     if (err.code != FLOCKGPU_ERR_UNSUPPORTED) throw;
     tree_pred = compile_tree_predicate(*predicate, infos);

@@ -686,7 +686,9 @@ static JoinCount join_count(const ExecEnv& env, const HashAggregateExec& agg, co
     emit_expr(*filter[fact]->predicate, *in[fact], &pred);
     std::vector<fg::ColInfo> infos;
     for (const fg::Column& c : in[fact]->cols) infos.push_back({c.dtype, c.name, c.format, c.validity != nullptr});
-    if (fg::compile_predicate(pred, infos).prog.has_div_by_col) {  // the filter reports a division by zero itself
+    // the filter reports a division by zero itself, and evaluates a CAST that can give NULL in the tree form
+    const fg::CompiledPredicate cp = fg::compile_predicate(pred, infos);
+    if (cp.prog.has_div_by_col || cp.lossy_cast) {
       in[fact] = filter[fact]->apply(env, in[fact]);
       filter[fact] = nullptr;
     }

@@ -5,6 +5,7 @@ The judge is a row-at-a-time restatement of the semantics in this file (`ref_eva
 wrapping integers, truncated division, one IEEE rounding per Float64 node, Kleene logic, SQL CASE and IN), itself checked
 against Arrow compute on the shapes Arrow compute expresses."""
 import math
+import re
 
 import numpy as np
 import pyarrow as pa
@@ -13,8 +14,10 @@ import pytest
 
 import flock_b200 as fb
 from flock_b200 import _ffi, col, lit, case
+from test_tpch_host import LIKE_PATTERNS
 
 I32, I64, U64, F64, TS, UTF8, BOOL = fb.INT32, fb.INT64, fb.UINT64, fb.FLOAT64, fb.TIMESTAMP, fb.UTF8, fb.BOOL
+U32, D32 = fb.UINT32, fb.DATE32
 
 
 # ---- the reference: a postfix stack machine over python values (value, is_null, divided_by_zero) ----------------------
@@ -23,7 +26,7 @@ class DivideByZero(Exception):
 
 
 def _wrap(v, dt):
-    if dt == I32:
+    if dt in (I32, D32):
         return ((int(v) + (1 << 31)) & 0xffffffff) - (1 << 31)
     if dt == fb.UINT32:
         return int(v) & 0xffffffff
@@ -44,13 +47,25 @@ def _promote(a, b):
     return a if _rank(a) >= _rank(b) else b
 
 
-def _convert(v, frm, to):
+_RANGE = {I32: (-(1 << 31), (1 << 31) - 1), U32: (0, (1 << 32) - 1), I64: (-(1 << 63), (1 << 63) - 1), TS: (-(1 << 63), (1 << 63) - 1),
+          U64: (0, (1 << 64) - 1)}
+
+
+def _convert(v, frm, to, cast=False):
+    """frm -> to.  Implicit conversions (coercion to a common type) wrap; an explicit CAST (cast=True) gives None where
+    `to` cannot hold the value, as arrow-rs's numeric cast (num::cast::cast) does: NaN, +-inf, a float out of range
+    once truncated toward zero, an integer out of range."""
     if frm == to or v is None or BOOL in (frm, to):
         return v
     if to == F64:
         return float(v)
     if frm == F64:
+        if not math.isfinite(v):
+            return None if cast else 0
         v = math.trunc(v)
+    if cast:
+        lo, hi = _RANGE[to]
+        return v if lo <= v <= hi else None
     return _wrap(v, to)
 
 
@@ -89,6 +104,12 @@ def _kleene(op, a, b):
     return (None, True, ea or eb, BOOL) if (na or nb) else (not dom, False, ea or eb, BOOL)
 
 
+def _like(s, pattern):
+    """SQL LIKE without an escape character: '%' any run of code points, '_' exactly one."""
+    rx = "".join(".*" if ch == "%" else "." if ch == "_" else re.escape(ch) for ch in pattern)
+    return re.fullmatch(rx, s, re.DOTALL) is not None
+
+
 def ref_eval_row(tokens, row, dtypes):
     st = []
     for op, dt, c, i64, f64, s in tokens:
@@ -104,7 +125,11 @@ def ref_eval_row(tokens, row, dtypes):
             st.append((None, True, False, dt))
         elif op == fb.OP_CAST:
             v, n, e, t = st.pop()
-            st.append((_convert(v, t, dt), n, e, dt))
+            v = _convert(v, t, dt, cast=True)
+            st.append((v, v is None, e, dt))
+        elif op in (fb.OP_LIKE, fb.OP_NOT_LIKE):
+            (p, np_, ep, _), (v, n, e, t) = st.pop(), st.pop()
+            st.append((None, True, e or ep, BOOL) if n or np_ else (_like(v, p) != (op == fb.OP_NOT_LIKE), False, e or ep, BOOL))
         elif op == fb.OP_NEG:
             v, n, e, t = st.pop()
             st.append((None if n else (-v if t == F64 else _wrap(-v, t)), n, e, t))
@@ -171,9 +196,10 @@ def ref_eval_row(tokens, row, dtypes):
 
 
 def ref_eval(e, batch):
-    dtypes = [{pa.int32(): I32, pa.int64(): I64, pa.uint64(): U64, pa.float64(): F64, pa.string(): UTF8}.get(f.type, TS) for f in batch.schema]
-    cols = [[v.value if hasattr(v, "value") and not isinstance(v, (int, float, str)) else v for v in c.to_pylist()] for c in
-            [pc.cast(c, pa.int64()) if pa.types.is_timestamp(c.type) else c for c in batch.columns]]
+    dtypes = [{pa.int32(): I32, pa.int64(): I64, pa.uint64(): U64, pa.uint32(): U32, pa.float64(): F64, pa.string(): UTF8, pa.date32(): D32}.get(f.type, TS)
+              for f in batch.schema]
+    cols = [c.to_pylist() for c in [pc.cast(c, pa.int64()) if pa.types.is_timestamp(c.type) else pc.cast(c, pa.int32()) if c.type == pa.date32() else c
+                                    for c in batch.columns]]
     out = []
     for r in range(batch.num_rows):
         v, n, err, t = ref_eval_row(fb.E.wrap(e).tokens, [c[r] for c in cols], dtypes)
@@ -211,17 +237,108 @@ def batch(n=64, seed=0, nulls=True):
     ], names=["a", "l", "u", "f", "t", "s", "z", "d"])
 
 
+# ---- the edge relation: the columns of batch() (same indices) plus UInt32, Date32 and a row id --------------------------
+I32_MIN, I32_MAX, I64_MIN, I64_MAX = -(1 << 31), (1 << 31) - 1, -(1 << 63), (1 << 63) - 1
+NEG_NAN = float(np.uint64(0xfff8000000000000).view(np.float64))
+EDGE_POOLS = [
+    [I32_MIN, I32_MAX, -1, 0, 1, I32_MIN + 1],                                                        # a   Int32
+    [I64_MIN, I64_MAX, -1, 0, (1 << 53) + 1, -(1 << 53) - 1, I64_MIN + 1],                            # l   Int64
+    [1 << 63, (1 << 64) - 1, 0, 1, (1 << 63) + 1, (1 << 63) - 1],                                      # u   UInt64
+    [0.0, -0.0, math.inf, -math.inf, math.nan, NEG_NAN, 5e-324, -5e-324, 1.5e-310, 1e308, -1e308, 0.1,
+     2.0 ** 63, -2.0 ** 63, 2.0 ** 64, 2147483647.9, -2147483648.9, 4294967295.5, -0.5, 9.3e18],        # f   Float64
+    [-1, -86_400_000 * 365 * 30 - 7, I64_MIN, I64_MAX, 0, -1_000_000_000_000_001],                    # t   Timestamp(ms), before 1970
+    ["", "é", "日本語", "a" * 70, "a" * 71, "PROMO", "PROMO BRUSHED", "PROMO BRUSHED TIN", "%", "_", "aé", "abab"],  # s   Utf8
+    [-1, 1, I32_MIN, -1, 1],                                                                          # z   Int32 divisor (no 0)
+    [0.0, -0.0, 0.1, 1e308, -5e-324],                                                                 # d   Float64
+    [1 << 31, (1 << 32) - 1, 0, (1 << 31) - 1, (1 << 31) + 1],                                        # w   UInt32
+    [0, -1, I32_MIN, I32_MAX, -719_162, 2_932_896],                                                   # day Date32
+]
+EDGE_BLOCK = 24                                 # rows of the fixed edge block: at the start, in the middle and at the end
+WORDS = ["MAIL", "SHIP", "AIR", "RAIL", "1-URGENT", "2-HIGH", "", "x", "PROMO PLATED", "STANDARD PROMO", "promo x", "éa", "a%b", "a_b",
+         "xxabxxab", "日本語"]
+NULLABLE = (0, 2, 3, 5, 8, 9)                   # a, u, f, s, w, day; the rest never hold NULLs
+
+
+def edge_relation(n, seed, nulls=7):
+    """`n` rows: ~30 % of each column from its edge pool, the rest ordinary; one fixed edge block at the start, in the
+    middle and in the last rows.  nulls: 0 none, 7 one row in 7, -1 every row but one (in the nullable columns)."""
+    rng = np.random.default_rng(seed)
+    ordinary = [rng.integers(-1000, 1000, n), rng.integers(-(1 << 40), 1 << 40, n), rng.integers(0, 1 << 64, n, dtype=np.uint64),
+                np.round(rng.normal(0, 100, n), 2), rng.integers(1_436_918_400_000, 1_436_918_500_000, n), None,
+                rng.choice([2, 3, -7, 1000, -1, 1], n), rng.integers(0, 11, n) / 100.0, rng.integers(0, 1 << 32, n, dtype=np.uint64),
+                rng.integers(8000, 11000, n)]
+    types = [np.int32, np.int64, np.uint64, np.float64, np.int64, object, np.int32, np.float64, np.uint32, np.int32]
+    arrow = [pa.int32(), pa.int64(), pa.uint64(), pa.float64(), pa.timestamp("ms"), pa.string(), pa.int32(), pa.float64(), pa.uint32(), pa.date32()]
+    starts = sorted({0, (n // 2) & ~3, max(n - EDGE_BLOCK, 0)})
+    arrays = []
+    for c, pool in enumerate(EDGE_POOLS):
+        pool = np.array(pool, dtype=object if types[c] in (object, np.uint64) else types[c])
+        if c == 5:
+            v = np.array(WORDS + EDGE_POOLS[5], dtype=object)[rng.integers(0, len(WORDS) + len(EDGE_POOLS[5]), n)]
+        else:
+            v = ordinary[c].astype(types[c])
+        edge = rng.random(n) < 0.3
+        v = v.astype(object) if types[c] is np.uint64 else v
+        v[edge] = pool[rng.integers(0, len(pool), int(edge.sum()))]
+        for s in starts:
+            k = min(EDGE_BLOCK, n - s)
+            v[s:s + k] = pool[(np.arange(k) + c) % len(pool)]
+        mask = None
+        if c in NULLABLE and nulls and n:
+            mask = rng.integers(0, nulls, n) == 0 if nulls > 0 else np.arange(n) != int(rng.integers(0, n))
+        arrays.append(pa.array(v if types[c] is not np.uint64 else v.tolist(), arrow[c], mask=mask))
+    arrays.append(pa.array(np.arange(n, dtype=np.int64)))
+    return pa.RecordBatch.from_arrays(arrays, names=["a", "l", "u", "f", "t", "s", "z", "d", "w", "day", "rid"])
+
+
 # ---- random trees ------------------------------------------------------------------------------------------------------
-def random_tree(rng, depth, kind):
-    """kind: 'int' | 'float' | 'bool'.  Float -> integer casts are left out (out-of-range conversions differ by platform)."""
+INT_TYPES = ("int32", "uint32", "int64", "uint64")
+
+
+def random_tree(rng, depth, kind, edges=False):
+    """kind: 'int' | 'float' | 'bool'.  edges=False: the columns of batch() and mild literals.  edges=True (the edge
+    relation): also UInt32 / Date32 columns, the edge literals, division by the divisor column, Int32 results that
+    wrap, comparisons across Int64 / UInt64 / Float64, NaN operands, explicit casts that can give NULL, CASE with a base
+    expression and LIKE."""
     pick = lambda *xs: xs[int(rng.integers(0, len(xs)))]
+    sub = lambda k: random_tree(rng, depth - 1, k, edges)
+    if edges and rng.random() < 0.3:
+        if depth == 0 or rng.random() < 0.4:
+            if kind == "int":
+                return pick(col(8), col(2), lit(I32_MIN, "int32"), lit(I32_MAX, "int32"), lit(I64_MIN), lit(I64_MAX), lit((1 << 53) + 1),
+                            lit((1 << 64) - 1, "uint64"), lit(1 << 31, "uint32"), lit(-1), col(3).cast(pick(*INT_TYPES)),
+                            col(1).cast(pick("int32", "uint32", "uint64")), col(2).cast(pick("int64", "int32")), col(8).cast("int32"),
+                            col(0).cast(pick("uint32", "uint64")))
+            if kind == "float":
+                return pick(col(3), lit(math.nan), lit(NEG_NAN), lit(math.inf), lit(-math.inf), lit(-0.0), lit(5e-324), lit(1e308), lit(-1e308),
+                            lit(0.1), col(2).cast("float64"), col(1).cast("float64"), col(8).cast("float64"))
+            return pick(col(3) == math.nan, col(3) < lit(NEG_NAN), col(3) != math.nan, col(5).like(pick(*LIKE_PATTERNS), rng.random() < 0.4),
+                        col(9) < lit(int(rng.integers(-2, 11000)), "date32"), col(9).isin([lit(0, "date32"), lit(-1, "date32"), lit(I32_MIN, "date32")]),
+                        col(1) < col(2), col(2) >= col(3), col(1) == col(3), col(8) > col(0), col(8) <= col(1))
+        r = rng.random()
+        if kind == "int":
+            if r < 0.3:
+                return pick(sub("int") / col(6), sub("int") % col(6), sub("int") / col(6).cast("int64"), sub("int") % col(6).cast("int64"))
+            if r < 0.5:
+                return pick(col(0) * col(0), col(0) + lit(I32_MAX, "int32"), -col(0), col(0) * col(6) - lit(I32_MIN, "int32"), col(8) * col(8))
+            if r < 0.75:
+                return pick(sub("float").cast(pick(*INT_TYPES)), sub("int").cast(pick("int32", "uint32", "uint64")))
+            return case([(int(rng.integers(-2, 3)), sub("int")), (lit(1 << 31, "uint32"), sub("int"))], base=pick(col(8), col(0), sub("int")),
+                        otherwise=sub("int") if rng.random() < 0.6 else None)
+        if kind == "float":
+            return pick(sub("float") / sub("float"), sub("float") * sub("int"), sub("int").cast("float64") - sub("float"))
+        if r < 0.5:
+            a, b = pick(sub("int"), sub("float"), col(2), col(8)), pick(sub("int"), sub("float"), col(2), col(1))
+            return pick(a == b, a != b, a < b, a <= b, a > b, a >= b)
+        if r < 0.7:
+            return col(5).like(pick(*LIKE_PATTERNS), rng.random() < 0.4) | sub("bool")
+        return pick(sub("int"), sub("float")).isin([I64_MIN, -1, None] if rng.random() < 0.5 else [0, 1 << 31], negated=rng.random() < 0.4)
     if depth == 0 or rng.random() < 0.15:
         if kind == "int":
             return pick(col(0), col(1), col(6), col(0).cast("int64"), lit(int(rng.integers(-9, 10))), col(4).cast("int64"))
         if kind == "float":
             return pick(col(3), col(7), lit(float(np.round(rng.normal(0, 5), 2))), col(0).cast("float64"))
         return pick(col(0) > int(rng.integers(-20, 20)), col(5) == pick("MAIL", "SHIP", ""), col(3).is_null(), col(7) <= 0.05, col(5) < "RAIL")
-    sub = lambda k: random_tree(rng, depth - 1, k)
     r = rng.random()
     if kind in ("int", "float"):
         if r < 0.5:
@@ -229,7 +346,7 @@ def random_tree(rng, depth, kind):
             ops = [lambda: a + b, lambda: a - b, lambda: a * b, lambda: a / b] + ([lambda: a % b] if kind == "int" else [])
             return ops[int(rng.integers(0, len(ops)))]()
         if r < 0.6:
-            return -sub(kind)
+            return -(sub(kind).cast("int64") if edges and kind == "int" else sub(kind))   # unary minus takes no unsigned operand
         if r < 0.85:
             n = int(rng.integers(1, 3))
             return case([(sub("bool"), sub(kind)) for _ in range(n)], otherwise=sub(kind) if rng.random() < 0.7 else None)
@@ -437,3 +554,112 @@ def test_old_forms_still_win():
         with pytest.raises(fb.FlockGpuError) as info:                        # the chain form keeps refusing what it refused
             fb.selftest_eval_value(b, e)
         assert info.value.code == _ffi.ERR_UNSUPPORTED
+
+
+# ---- the edge relation: the host interpreter against the reference, the reference against Arrow compute ----------------
+def run_tree(b, e, kind):
+    """The host build of the tree form: ('ok', mask | (values, valid, dtype)), ('refused', None) for a tree over the
+    compiler's register / instruction budget, ('raised', None) for "Divide by zero"."""
+    try:
+        if kind == "bool":
+            return "ok", fb.selftest_eval_tree(b, e, predicate=True)[0]
+        return "ok", fb.selftest_eval_tree(b, [e])[0][0]
+    except fb.FlockGpuError as err:
+        if err.code == _ffi.ERR_UNSUPPORTED and ("registers" in err.message or "instructions" in err.message):
+            return "refused", None
+        assert err.code == _ffi.ERR_EXECUTION and "Divide by zero" in err.message, (err, e.tokens)
+        return "raised", None
+
+
+def check_against_reference(b, e, kind, got):
+    """`got` (run_tree over `b`) against ref_eval over the same rows."""
+    status, res = got
+    try:
+        want = ref_eval(e, b)
+    except DivideByZero:
+        assert status == "raised", e.tokens
+        return
+    assert status == "ok", (status, e.tokens)
+    if kind == "bool":
+        assert list(res) == [w is True for w in want], e.tokens
+    elif res[0] is not None:
+        same(res[0], res[1], want, res[2])
+
+
+@pytest.mark.parametrize("seed", [42, 7, 1234])
+def test_random_edge_trees_match_the_reference(seed):
+    rng = np.random.default_rng(seed)
+    counts = {"ok": 0, "refused": 0, "raised": 0}
+    for k in range(90):
+        b = edge_relation(300, seed=seed * 1000 + k, nulls=[0, 7, -1][k % 3])
+        kind = ["int", "float", "bool"][k % 3]
+        e = random_tree(rng, int(rng.integers(2, 6)), kind, edges=True)
+        got = run_tree(b, e, kind)
+        counts[got[0]] += 1
+        if got[0] != "refused":
+            check_against_reference(b, e, kind, got)
+    assert counts["ok"] >= 55 and counts["refused"] <= 20, counts
+
+
+def test_edge_reference_agrees_with_arrow_compute():
+    b = edge_relation(400, seed=3)
+    A, L, U, F, S, W = (b.column(i) for i in (0, 1, 2, 3, 5, 8))
+    keep = lambda e: [w is True for w in ref_eval(e, b)]
+    arrow = lambda x: [w is True for w in x.to_pylist()]
+    for p in LIKE_PATTERNS:
+        for negated in (False, True):
+            want = pc.match_like(S, p)
+            assert keep(col(5).like(p, negated)) == arrow(pc.invert(want) if negated else want), p
+    P, Q = col(0) > 0, col(3) < 0.5
+    AP, AQ = pc.greater(A, 0), pc.less(F, 0.5)
+    for e, x in [(P & Q, pc.and_kleene(AP, AQ)), (P | Q, pc.or_kleene(AP, AQ)), (~(P & ~Q), pc.invert(pc.and_kleene(AP, pc.invert(AQ)))),
+                 (col(1).isin([I64_MIN, -1, 0, (1 << 53) + 1]), pc.is_in(L, value_set=pa.array([I64_MIN, -1, 0, (1 << 53) + 1]))),
+                 (col(8).isin([lit(1 << 31, "uint32"), lit(0, "uint32")]), pc.is_in(W, value_set=pa.array([1 << 31, 0], pa.uint32()))),
+                 (col(2).isin([lit((1 << 64) - 1, "uint64")]), pc.is_in(U, value_set=pa.array([(1 << 64) - 1], pa.uint64()))),
+                 (col(3) == math.nan, pc.equal(F, math.nan)), (col(3) >= 0.1, pc.greater_equal(F, 0.1))]:
+        assert keep(e) == arrow(x), e.tokens
+    # Int32 arithmetic wraps (arrow's unchecked kernels); the integer CASTs agree with Arrow's checked cast (Arrow's
+    # Float64 -> integer cast cannot be the judge: it truncates only with its range check switched off)
+    assert ref_eval(col(0) * col(0), b) == pc.multiply(A, A).to_pylist()
+    for src, to, dt in [(1, "int32", pa.int32()), (2, "int64", pa.int64()), (8, "int32", pa.int32()), (0, "uint64", pa.uint64())]:
+        got = ref_eval(col(src).cast(to), b)
+        for r, v in enumerate(got):
+            w = b.column(src).slice(r, 1)
+            if v is not None:
+                assert [v] == pc.cast(w, dt).to_pylist()
+            elif w.null_count == 0:                                        # NULL only where Arrow's checked cast refuses the value
+                with pytest.raises(pa.ArrowInvalid):
+                    pc.cast(w, dt)
+
+
+def test_lossy_cast_is_null_in_the_tree_form():
+    """CAST(Float64 AS an integer type) and narrowing integer CASTs: NULL where the target cannot hold the value
+    (arrow-rs's numeric cast), truncation toward zero otherwise.  The chain form lowers the same cast without its NULLs
+    (the operators evaluate such an expression in the tree form): it agrees wherever the value fits."""
+    f = [0.0, -0.0, math.inf, -math.inf, math.nan, NEG_NAN, 2.5, -2.5, 2147483647.9, 2147483648.0, -2147483648.9, -2147483649.0, -0.5, -1.0,
+         4294967295.5, 4294967296.0, 2.0 ** 63, -2.0 ** 63, 9223372036854774784.0, 2.0 ** 64, 18446744073709549568.0, 1e308, 5e-324]
+    i = [0, -1, I32_MIN, I32_MAX, I32_MAX + 1, I32_MIN - 1, (1 << 32) - 1, 1 << 32, I64_MIN, I64_MAX]
+    u = [0, 1, I32_MAX, 1 << 31, (1 << 32) - 1, 1 << 32, I64_MAX, 1 << 63, (1 << 64) - 1, 5]
+    b = pa.record_batch([pa.array(f), pa.array(i + [7] * (len(f) - len(i))), pa.array(u + [7] * (len(f) - len(u)), pa.uint64())], ["f", "i", "u"])
+    fits = {"int32": lambda v: I32_MIN <= v <= I32_MAX, "uint32": lambda v: 0 <= v < 1 << 32, "int64": lambda v: I64_MIN <= v <= I64_MAX,
+            "uint64": lambda v: 0 <= v < 1 << 64}
+    for src in range(3):
+        for to in INT_TYPES:
+            e = col(src).cast(to)
+            want = ref_eval(e, b)
+            for v, w in zip(b.column(src).to_pylist(), want):
+                t = math.trunc(v) if isinstance(v, float) and math.isfinite(v) else v
+                assert w == (t if isinstance(t, int) and fits[to](t) else None), (src, to, v, w)
+            if src == 1 and to == "int64" or src == 2 and to == "uint64":
+                continue                                                   # no cast at all: a plain column
+            (vals, valid, dt), = fb.selftest_eval_tree(b, [e])[0]
+            same(vals, valid, want, dt)
+            mask, _ = fb.selftest_eval_tree(b, e.is_null(), predicate=True)         # IS NULL sees the NULLs of the cast
+            assert list(mask) == [w is None for w in want]
+            chain, cdt = fb.selftest_eval_value(b, e)
+            assert cdt == dt and all(int(c) == (w & ((1 << 64) - 1) if to == "uint64" else w) for c, w in zip(chain, want) if w is not None)
+    # widening casts and implicit coercion keep wrapping, and keep the chain form
+    v, dt = fb.selftest_eval_value(b, col(1).cast("float64") + col(2).cast("float64"))
+    assert dt == F64
+    v, dt = fb.selftest_eval_value(b, col(1) + col(2))                     # Int64 + UInt64: both as UInt64, wrapping
+    assert dt == U64 and [int(x) for x in v] == [(x + y) & ((1 << 64) - 1) for x, y in zip(b.column(1).to_pylist(), b.column(2).to_pylist())]
