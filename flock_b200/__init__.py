@@ -35,8 +35,10 @@ OP_ADD, OP_SUB, OP_MUL, OP_DIV, OP_MOD = 10, 11, 12, 13, 14
 OP_EQ, OP_NE, OP_LT, OP_LE, OP_GT, OP_GE = 20, 21, 22, 23, 24, 25
 OP_AND, OP_OR, OP_NOT = 30, 31, 32
 OP_NEG, OP_IS_NULL, OP_IS_NOT_NULL, OP_LIT_NULL, OP_CASE, OP_IN_LIST = 40, 41, 42, 43, 44, 45
-OP_LIKE, OP_NOT_LIKE = 46, 47
+OP_LIKE, OP_NOT_LIKE, OP_DATE_PART = 46, 47, 48
 CASE_HAS_BASE, CASE_HAS_ELSE = 1, 2
+DATE_PART_YEAR, DATE_PART_HOUR = 1, 2
+_DATE_PART_BY_NAME = {"year": DATE_PART_YEAR, "hour": DATE_PART_HOUR}
 # enum flockgpu_agg_mode / flockgpu_agg_func
 AGG_PARTIAL, AGG_FINAL, AGG_FINAL_PARTITIONED, AGG_SINGLE = 0, 1, 2, 3
 AGG_COUNT, AGG_SUM, AGG_MIN, AGG_MAX, AGG_AVG = 0, 1, 2, 3, 4
@@ -95,6 +97,11 @@ class E:
     def like(self, pattern, negated: bool = False) -> "E":
         """self [NOT] LIKE pattern (a str, or None for a NULL pattern)."""
         return self._bin(OP_NOT_LIKE if negated else OP_LIKE, null("utf8") if pattern is None else pattern)
+
+    def extract(self, field: str | int) -> "E":
+        """EXTRACT(field FROM self), DataFusion's date_part: "year" / "hour" (any case) or a DATE_PART_* code.  Int32."""
+        code = _DATE_PART_BY_NAME[field.lower()] if isinstance(field, str) else int(field)
+        return E(self.tokens + [(OP_DATE_PART, 0, code, 0, 0.0, None)])
 
     def isin(self, values, negated: bool = False) -> "E":
         """self [NOT] IN (values): literals (None = a NULL literal)."""

@@ -73,6 +73,35 @@ struct Tree {
   int root = -1;
 };
 
+// The unit of date_part's Timestamp operand `idx`: that of the first Timestamp column it reads, as compile_value keeps
+// the format of a computed Timestamp.  A timezone, or no Timestamp column at all (a literal), is refused.
+int timestamp_unit(const Tree& t, int idx, const std::vector<ColInfo>& cols) {
+  std::function<int(int)> first = [&](int i) -> int {
+    if (i < 0) return -1;
+    const Node& x = t.nodes[i];
+    if (x.op == FLOCKGPU_OP_COLUMN) return x.dtype == FLOCKGPU_TIMESTAMP ? x.col : -1;
+    for (int k : {x.l, x.r})
+      if (int c = first(k); c >= 0) return c;
+    for (int k : x.kids)
+      if (int c = first(k); c >= 0) return c;
+    return -1;
+  };
+  const int c = first(idx);
+  FG_CHECK(c >= 0, FLOCKGPU_ERR_UNSUPPORTED, "expression: date_part of a Timestamp that reads no Timestamp column (its unit is unknown)");
+  const std::string& f = cols[c].format;  // "ts" + unit letter + ':' + timezone
+  FG_CHECK(f.size() >= 4 && f.compare(0, 2, "ts") == 0 && f[3] == ':', FLOCKGPU_ERR_INVALID, "expression: Timestamp column \"%s\" has format \"%s\"",
+           cols[c].name.c_str(), f.c_str());
+  FG_CHECK(f.size() == 4, FLOCKGPU_ERR_UNSUPPORTED, "expression: date_part of Timestamp with timezone %s (column \"%s\")", f.c_str() + 4,
+           cols[c].name.c_str());
+  switch (f[2]) {
+    case 's': return DU_S;
+    case 'm': return DU_MS;
+    case 'u': return DU_US;
+    case 'n': return DU_NS;
+  }
+  fail(FLOCKGPU_ERR_INVALID, "expression: Timestamp column \"%s\" has format \"%s\"", cols[c].name.c_str(), f.c_str());
+}
+
 Tree build_tree(const Expr& e, const std::vector<ColInfo>& cols) {
   Tree t;
   std::vector<int> stack;
@@ -194,6 +223,17 @@ Tree build_tree(const Expr& e, const std::vector<ColInfo>& cols) {
         FG_CHECK(v.dtype == FLOCKGPU_UTF8 || v.op == FLOCKGPU_OP_LIT_NULL, FLOCKGPU_ERR_UNSUPPORTED, "expression: LIKE over %s", dtype_name(v.dtype));
         FG_CHECK(pat.op == FLOCKGPU_OP_LIT_UTF8 || pat.op == FLOCKGPU_OP_LIT_NULL, FLOCKGPU_ERR_UNSUPPORTED, "expression: LIKE needs a literal pattern");
         n.dtype = FLOCKGPU_BOOL;
+        break;
+      }
+      case FLOCKGPU_OP_DATE_PART: {
+        n.l = pop();
+        n.flags = tok.col;
+        FG_CHECK(tok.col == FLOCKGPU_DATE_PART_YEAR || tok.col == FLOCKGPU_DATE_PART_HOUR, FLOCKGPU_ERR_UNSUPPORTED,
+                 "expression: date_part field %d (YEAR and HOUR only)", tok.col);
+        const int xt = t.nodes[n.l].dtype;
+        FG_CHECK(xt == FLOCKGPU_DATE32 || xt == FLOCKGPU_TIMESTAMP, FLOCKGPU_ERR_UNSUPPORTED, "expression: date_part of %s", dtype_name(xt));
+        n.i = xt == FLOCKGPU_DATE32 ? DU_DAY : timestamp_unit(t, n.l, cols);
+        n.dtype = FLOCKGPU_INT32;
         break;
       }
       default:
@@ -362,6 +402,7 @@ struct ChainBuilder {
       convert(c, t.nodes[n.l].dtype, n.dtype);
       return c;
     }
+    FG_CHECK(n.op != FLOCKGPU_OP_DATE_PART, FLOCKGPU_ERR_UNSUPPORTED, "expression: date_part runs in the tree form only");
     FG_CHECK(is_arith(n.op), FLOCKGPU_ERR_UNSUPPORTED, "expression: boolean sub-expression used as a value");
     int T = n.dtype;
     bool is_col = false;
@@ -857,6 +898,17 @@ struct TreeBuilder {
         id = intern(x);
         break;
       }
+      case FLOCKGPU_OP_DATE_PART: {
+        TNode x;
+        x.op = T_DATE_PART;
+        x.sub = n.flags;
+        x.a = lower(t, n.l, memo);
+        x.lit.i = n.i;
+        // only a year of seconds can leave Int32: 2^31 years are some 6.8e16 s
+        x.may_null = nullable(x.a) || (n.flags == FLOCKGPU_DATE_PART_YEAR && n.i == DU_S);
+        id = intern(x);
+        break;
+      }
       case FLOCKGPU_OP_IN_LIST: {
         // x IN (a, b) is x = a OR x = b under Kleene's OR: exactly SQL's three-valued IN
         for (size_t k = 1; k < n.kids.size(); ++k) {
@@ -1073,6 +1125,12 @@ std::string expr_to_string(const Expr& e, const std::vector<ColInfo>& cols) {
         if (has_else) s += "ELSE " + st.back() + " ";
         st.resize(at);
         st.push_back(s + "END");
+        break;
+      }
+      case FLOCKGPU_OP_DATE_PART: {
+        if (st.empty()) return "<malformed>";
+        std::string a = st.back(); st.pop_back();
+        st.push_back(std::string("date_part(") + (t.col == FLOCKGPU_DATE_PART_HOUR ? "HOUR" : t.col == FLOCKGPU_DATE_PART_YEAR ? "YEAR" : "?") + ", " + a + ")");
         break;
       }
       case FLOCKGPU_OP_IN_LIST: {

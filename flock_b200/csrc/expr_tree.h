@@ -39,7 +39,8 @@ enum TreeOp : int16_t {
   T_IS_NULL, T_IS_NOT_NULL,
   T_SELECT,       // r[d] = r[c] is TRUE ? r[a] : r[b]   (a NULL condition takes r[b]: CASE falls through)
   T_STORE,        // output `col` = r[a]
-  T_LIKE          // r[d] = Utf8 column `col` LIKE pooled pattern lit (offset << 32 | length); sub = 1: NOT LIKE
+  T_LIKE,         // r[d] = Utf8 column `col` LIKE pooled pattern lit (offset << 32 | length); sub = 1: NOT LIKE
+  T_DATE_PART     // r[d] = date_part(sub = FLOCKGPU_DATE_PART_*, r[a]); lit = the operand's unit (DateUnit)
 };
 
 constexpr uint8_t TF_NULL = 1, TF_ERR = 2;
@@ -105,6 +106,50 @@ FG_HD bool like_match(const uint8_t* s, int n, const uint8_t* p, int m) {
   }
   while (pi < m && p[pi] == '%') ++pi;
   return pi == m;
+}
+
+// The unit of a date_part operand: a Date32 counts days, a Timestamp seconds, milli-, micro- or nanoseconds.
+enum DateUnit : int { DU_DAY = 0, DU_S, DU_MS, DU_US, DU_NS };
+
+// Proleptic Gregorian year of `day` (days since 1970-01-01), year 0 included: civil_from_days (H. Hinnant), the
+// inverse of the plan reader's days_from_civil, in 64-bit so that every day an Int64 timestamp can name is exact.
+FG_HD int64_t year_of_day(int64_t day) {
+  const int64_t z = day + 719468;
+  const int64_t era = (z >= 0 ? z : z - 146096) / 146097;
+  const int64_t doe = z - era * 146097;                                    // [0, 146096]
+  const int64_t yoe = (doe - doe / 1460 + doe / 36524 - doe / 146096) / 365;  // [0, 399]
+  const int64_t doy = doe - (365 * yoe + yoe / 4 - yoe / 100);             // [0, 365], from March 1st
+  const int64_t mp = (5 * doy + 2) / 153;                                  // [0, 11], March = 0
+  return yoe + era * 400 + (mp >= 10);                                     // January and February close the year
+}
+
+// date_part(field, v) for v counted in units of which PER_DAY make a day and PER_HOUR an hour.  The day is the floor
+// of v / PER_DAY, so an instant before 1970 falls on its own day.  false: the result is NULL (a year beyond Int32).
+template <int64_t PER_DAY, int64_t PER_HOUR>
+FG_HD bool date_part_in(int field, int64_t v, int64_t* out) {
+  int64_t day = v / PER_DAY, rem = v % PER_DAY;
+  if (rem < 0) {
+    --day;
+    rem += PER_DAY;
+  }
+  if (field == FLOCKGPU_DATE_PART_HOUR) {
+    *out = rem / PER_HOUR;
+    return true;
+  }
+  const int64_t y = year_of_day(day);
+  *out = y;
+  return y >= INT32_MIN && y <= INT32_MAX;
+}
+
+// One switch on the unit, so that every divisor is a compile-time constant.
+FG_HD bool date_part(int field, int unit, int64_t v, int64_t* out) {
+  switch (unit) {
+    case DU_S: return date_part_in<86400, 3600>(field, v, out);
+    case DU_MS: return date_part_in<86400000, 3600000>(field, v, out);
+    case DU_US: return date_part_in<86400000000ll, 3600000000ll>(field, v, out);
+    case DU_NS: return date_part_in<86400000000000ll, 3600000000000ll>(field, v, out);
+    default: return date_part_in<1, 1>(field, v, out);
+  }
 }
 
 // Runs the program for R rows (rows[j] < 0: no row); returns bit j = the verdict register is TRUE for row j.
@@ -245,6 +290,20 @@ FG_HD unsigned eval_tree(const TreeProgram& p, const ColRef* cols, const TreeOut
         }
         break;
       }
+      case T_DATE_PART:
+#pragma unroll
+        for (int j = 0; j < R; ++j) {
+          uint8_t f = rf.flag(in.a, j);
+          Val v;
+          v.i = 0;
+          if (!(f & TF_NULL) && !date_part(in.sub, int(in.lit.i), rf.val(in.a, j).i, &v.i)) {
+            v.i = 0;
+            f |= TF_NULL;
+          }
+          rf.val(in.d, j) = v;
+          rf.flag(in.d, j) = f;
+        }
+        break;
       case T_AND:
       case T_OR:
 #pragma unroll

@@ -315,28 +315,28 @@ __global__ void __launch_bounds__(256) join_emit_kernel(const __grid_constant__ 
 }
 
 // ------------------------------------------------------------------------------------------------
+// The kernels read the key columns only, so a side carries those alone: key i in slot i.  The other columns of the side,
+// however many, reach the output through gather_columns.
 static void fill_side(const Table& t, const std::vector<int>& keys, bool packed, JoinSide* s) {
-  FG_CHECK(t.cols.size() <= size_t(MAX_IN_COLS), FLOCKGPU_ERR_UNSUPPORTED, "hash_join: more than %d columns on one side", MAX_IN_COLS);
   s->n_rows = t.num_rows;
   s->packed = packed ? 1 : 0;
-  for (size_t i = 0; i < t.cols.size(); ++i) {
-    s->cols[i].data = t.cols[i].values();
-    s->cols[i].offsets = t.cols[i].offs();
-    s->cols[i].dtype = t.cols[i].dtype;
-    s->cols[i].chunk_shift = 0;
-    s->cols[i].chunks = nullptr;
-    s->cols[i].validity = nullptr;  // key equality between the sides is value equality: rows with NULL keys are skipped up front
-  }
   s->rk.n = int(keys.size());
   s->n_null_cols = 0;
   for (size_t i = 0; i < keys.size(); ++i) {
-    s->rk.col[i] = keys[i];
-    if (t.cols[keys[i]].validity) s->key_valid[s->n_null_cols++] = t.cols[keys[i]].valid();
+    const Column& c = t.cols[keys[i]];
+    s->cols[i].data = c.values();
+    s->cols[i].offsets = c.offs();
+    s->cols[i].dtype = c.dtype;
+    s->cols[i].chunk_shift = 0;
+    s->cols[i].chunks = nullptr;
+    s->cols[i].validity = nullptr;  // key equality between the sides is value equality: rows with NULL keys are skipped up front
+    s->rk.col[i] = int(i);
+    if (c.validity) s->key_valid[s->n_null_cols++] = c.valid();
   }
   if (packed) {
     s->pack.n = int(keys.size());
     for (size_t i = 0; i < keys.size(); ++i) {
-      s->pack.col[i] = keys[i];
+      s->pack.col[i] = int(i);
       s->pack.width[i] = t.cols[keys[i]].width();
     }
   }

@@ -3,6 +3,7 @@
 #include "plan.h"
 
 #include <algorithm>
+#include <cctype>
 #include <deque>
 #include <set>
 
@@ -164,6 +165,44 @@ static int binary_op(const std::string& op) {
   fail(FLOCKGPU_ERR_UNSUPPORTED, "plan: binary operator %s", op.c_str());
 }
 
+static bool is_scalar_function(const std::string& kind) { return kind == "scalar_function_expr" || kind == "scalar_function"; }
+
+// SQL's EXTRACT(f FROM x), which DataFusion 6 plans as the scalar function date_part(Utf8('f'), x): the
+// FLOCKGPU_DATE_PART_* code of its field.  date_part is the only scalar function of the GPU path; any other is refused
+// by name, as is a field other than YEAR or HOUR (matched in any case).
+static int date_part_field(const Json& e) {
+  const Json* fun = e.get("fun");
+  const Json* name = e.get("name");
+  const bool by_fun = fun && fun->is_string();
+  const std::string fname = by_fun ? fun->str : name && name->is_string() ? name->str : "?";
+  if (by_fun ? fname != "DatePart" : fname != "date_part" && fname != "datepart")
+    fail(FLOCKGPU_ERR_UNSUPPORTED, "plan: scalar function %s is not supported on the GPU path (date_part only)", fname.c_str());
+  const Json* args = e.get("args");
+  if (!args || !args->is_array() || args->arr.size() != 2) fail(FLOCKGPU_ERR_INVALID, "plan JSON: date_part takes two arguments");
+  const Json& f = *args->arr[0];
+  const Json* fk = f.get("physical_expr");
+  const Json* fv = f.get("value");
+  if (!fk || !fk->is_string() || fk->str != "literal" || !fv || !fv->is_object() || fv->obj.size() != 1 ||
+      (fv->obj[0].first != "Utf8" && fv->obj[0].first != "LargeUtf8") || !fv->obj[0].second->is_string())
+    fail(FLOCKGPU_ERR_UNSUPPORTED, "plan: date_part needs a Utf8 literal field");
+  std::string field = fv->obj[0].second->str;
+  for (char& c : field) c = char(toupper(static_cast<unsigned char>(c)));
+  if (field == "YEAR") return FLOCKGPU_DATE_PART_YEAR;
+  if (field == "HOUR") return FLOCKGPU_DATE_PART_HOUR;
+  fail(FLOCKGPU_ERR_UNSUPPORTED, "plan: date_part field %s is not supported on the GPU path (YEAR and HOUR only)", fv->obj[0].second->str.c_str());
+}
+
+// Every scalar function of a plan is checked when the plan is read, so that an unsupported one fails the unmarshal.
+static void check_scalar_functions(const Json& j) {
+  if (j.is_object()) {
+    const Json* k = j.get("physical_expr");
+    if (k && k->is_string() && is_scalar_function(k->str)) date_part_field(j);
+    for (const auto& kv : j.obj) check_scalar_functions(*kv.second);
+  } else if (j.is_array()) {
+    for (const JsonPtr& x : j.arr) check_scalar_functions(*x);
+  }
+}
+
 static void emit_expr(const Json& e, const fg::Table& in, Expr* out) {
   const std::string& kind = e.at("physical_expr").as_string("physical_expr tag");
   if (kind == "column") {
@@ -246,6 +285,12 @@ static void emit_expr(const Json& e, const fg::Table& in, Expr* out) {
     t.i64 = int64_t(list.arr.size());
     const Json* neg = e.get("negated");
     t.col = neg && neg->kind == Json::Bool && neg->b ? 1 : 0;
+    out->push_back(t);
+  } else if (is_scalar_function(kind)) {
+    ExprTok t{};
+    t.op = FLOCKGPU_OP_DATE_PART;
+    t.col = date_part_field(e);
+    emit_expr(*e.at("args").arr[1], in, out);
     out->push_back(t);
   } else {
     fail(FLOCKGPU_ERR_UNSUPPORTED, "plan: physical expression \"%s\" is not supported on the GPU path", kind.c_str());
@@ -398,6 +443,11 @@ static std::string expr_display(const Json& e) {
       for (size_t i = 0; i < list->arr.size(); ++i) s += (i ? ", " : "") + expr_display(*list->arr[i]);
     return s + "])";
   }
+  if (is_scalar_function(kind)) {
+    const Json* args = e.get("args");
+    if (!args || !args->is_array() || args->arr.size() != 2) return kind;
+    return "date_part(" + expr_display(*args->arr[0]) + ", " + expr_display(*args->arr[1]) + ")";
+  }
   return kind;
 }
 
@@ -471,12 +521,32 @@ TablePtr ProjectionExec::execute(const ExecEnv& env) {
     projs.push_back(std::move(t));
     names.push_back(e.second);
   }
-  if (filter) {
-    Expr pred;
-    emit_expr(*filter->predicate, *in, &pred);
-    return fg::filter_project(env.ctx, in, &pred, projs, names);
+  Expr pred;
+  if (filter) emit_expr(*filter->predicate, *in, &pred);
+  if (in->cols.size() > size_t(fg::MAX_IN_COLS)) {
+    // An input wider than one kernel argument block (TPC-H q8's and q9's subqueries over a 20- and a 17-column join)
+    // is narrowed to the columns the programs read, as views.  The tokens are remapped by index, not resolved again
+    // by name: q7 reads two columns named n_name.
+    in->resolve();
+    std::vector<Expr*> progs{&pred};
+    for (Expr& p : projs) progs.push_back(&p);
+    std::vector<int> at(in->cols.size(), -1);
+    for (const Expr* e : progs)
+      for (const ExprTok& t : *e)
+        if (t.op == FLOCKGPU_OP_COLUMN) at[t.col] = 0;
+    auto narrow = std::make_shared<fg::Table>(*in);
+    narrow->cols.clear();
+    for (size_t c = 0; c < in->cols.size(); ++c)
+      if (at[c] == 0) {
+        at[c] = int(narrow->cols.size());
+        narrow->cols.push_back(in->cols[c]);
+      }
+    for (Expr* e : progs)
+      for (ExprTok& t : *e)
+        if (t.op == FLOCKGPU_OP_COLUMN) t.col = at[t.col];
+    in = narrow;
   }
-  return fg::filter_project(env.ctx, in, nullptr, projs, names);
+  return fg::filter_project(env.ctx, in, filter ? &pred : nullptr, projs, names);
 }
 
 std::string FilterExec::fmt_as() const { return "FilterExec: " + expr_display(*predicate); }
@@ -684,6 +754,14 @@ static JoinCount join_count(const ExecEnv& env, const HashAggregateExec& agg, co
   Expr pred;
   if (filter[fact]) {
     emit_expr(*filter[fact]->predicate, *in[fact], &pred);
+    // dim_count interprets the term form, which has no date_part: such a predicate runs as its own filter first
+    if (std::any_of(pred.begin(), pred.end(), [](const ExprTok& t) { return t.op == FLOCKGPU_OP_DATE_PART; })) {
+      in[fact] = filter[fact]->apply(env, in[fact]);
+      filter[fact] = nullptr;
+      pred.clear();
+    }
+  }
+  if (filter[fact]) {
     std::vector<fg::ColInfo> infos;
     for (const fg::Column& c : in[fact]->cols) infos.push_back({c.dtype, c.name, c.format, c.validity != nullptr});
     // the filter reports a division by zero itself, and evaluates a CAST that can give NULL in the tree form
@@ -1023,6 +1101,7 @@ std::unique_ptr<ExecutionContext> ExecutionContext::unmarshal(const CtxPtr& ctx,
     fail(FLOCKGPU_ERR_INVALID, "unmarshal: expected a plan object, an array of plans or an ExecutionContext object");
   }
   if (plans.empty()) fail(FLOCKGPU_ERR_INVALID, "unmarshal: no execution plans");
+  check_scalar_functions(*root);
   for (const Json* p : plans) ec->execution_plans.push_back(build_plan(*p));
   return ec;
 }

@@ -84,6 +84,13 @@ def negative(arg: dict) -> dict:
     return {"physical_expr": "negative_expr", "arg": arg}
 
 
+def date_part(field: str, expr: dict) -> dict:
+    """SQL's EXTRACT(field FROM expr) as DataFusion 6 plans it: ScalarFunctionExpr date_part(Utf8(field), expr) -> Int32.
+    No fixture of the reference serialises a scalar function; the tag and fields follow the struct's as above."""
+    return {"physical_expr": "scalar_function_expr", "fun": "DatePart", "name": "date_part", "args": [literal("Utf8", field), expr],
+            "return_type": "Int32"}
+
+
 # ---- execution plans -------------------------------------------------------------------------------------
 def memory_exec(schema: pa.Schema, projection: list[int] | None) -> dict:
     return {"execution_plan": "memory_exec", "schema": schema_json(schema), "projection": projection}
@@ -614,3 +621,95 @@ TPCH_QUERIES = {"q1": tpch_q1, "q3": tpch_q3, "q5": tpch_q5, "q6": tpch_q6, "q10
 TPCH_SOURCES = {"q1": ["lineitem"], "q3": ["customer", "orders", "lineitem"],
                 "q5": ["customer", "orders", "lineitem", "supplier", "nation", "region"], "q6": ["lineitem"],
                 "q10": ["customer", "orders", "lineitem", "nation"], "q12": ["lineitem", "orders"], "q14": ["lineitem", "part"]}
+
+
+# ---- TPC-H q7, q8 and q9: EXTRACT(YEAR ...) and joins of up to 20 columns -------------------------------------------------
+# Shape unverified, like the queries above.  q8 and q9 list part and supplier first with no key between them, which
+# DataFusion 6's FROM-order planner would join as a cross join; the plans here join in FROM order except that part
+# follows lineitem, the first relation it has a key with.  BETWEEN is written as >= AND <=.
+def _between(e: dict, lo: str, hi: str) -> dict:
+    return _and(binary(e, "GtEq", _date(lo)), binary(e, "LtEq", _date(hi)))
+
+
+def _subquery(r: _Rel, exprs: list[tuple[dict, str]]) -> _Rel:
+    return _Rel(projection_exec(exprs, r.plan), [nm for _, nm in exprs])
+
+
+def tpch_q7(n: int = TARGET_PARTITIONS) -> dict:
+    su = _tpch_scan("supplier", ["s_suppkey", "s_nationkey"], n)
+    li = _filter(_tpch_scan("lineitem", ["l_orderkey", "l_suppkey", "l_extendedprice", "l_discount", "l_shipdate"], n),
+                 lambda r: _between(r.c("l_shipdate"), "1995-01-01", "1996-12-31"))
+    od = _tpch_scan("orders", ["o_orderkey", "o_custkey"], n)
+    cu = _tpch_scan("customer", ["c_custkey", "c_nationkey"], n)
+    n1 = _tpch_scan("nation", ["n_nationkey", "n_name"], n)
+    n2 = _tpch_scan("nation", ["n_nationkey", "n_name"], n)
+    j = _join(su, li, [("s_suppkey", "l_suppkey")], n)
+    j = _join(j, od, [("l_orderkey", "o_orderkey")], n)
+    j = _join(j, cu, [("o_custkey", "c_custkey")], n)
+    j = _join(j, n1, [("s_nationkey", "n_nationkey")], n)
+    j = _join(j, n2, [("c_nationkey", "n_nationkey")], n)
+    # two columns are named n_name: n1's comes first, n2's is the last
+    sn, cn = column("n_name", j.names.index("n_name")), column("n_name", len(j.names) - 1)
+    fr, de = literal("Utf8", "FRANCE"), literal("Utf8", "GERMANY")
+    j = _Rel(coalesce_batches_exec(filter_exec(binary(_and(binary(sn, "Eq", fr), binary(cn, "Eq", de)), "Or",
+                                                      _and(binary(sn, "Eq", de), binary(cn, "Eq", fr))), j.plan)), j.names)
+    shipping = _subquery(j, [(sn, "supp_nation"), (cn, "cust_nation"), (date_part("YEAR", j.c("l_shipdate")), "l_year"),
+                             (_revenue(j), "volume")])
+    rev = _sum("SUM(shipping.volume)", shipping.c("volume"))
+    g = _grouped(shipping, ["supp_nation", "cust_nation", "l_year"], [rev], n)
+    return _project_sort(g, [(g.c("supp_nation"), "supp_nation"), (g.c("cust_nation"), "cust_nation"), (g.c("l_year"), "l_year"),
+                             (g.c(rev["name"]), "revenue")], [("supp_nation", False), ("cust_nation", False), ("l_year", False)])
+
+
+def tpch_q8(n: int = TARGET_PARTITIONS) -> dict:
+    su = _tpch_scan("supplier", ["s_suppkey", "s_nationkey"], n)
+    li = _tpch_scan("lineitem", ["l_orderkey", "l_partkey", "l_suppkey", "l_extendedprice", "l_discount"], n)
+    pt = _filter(_tpch_scan("part", ["p_partkey", "p_type"], n), lambda r: binary(r.c("p_type"), "Eq", literal("Utf8", "ECONOMY ANODIZED STEEL")))
+    od = _filter(_tpch_scan("orders", ["o_orderkey", "o_custkey", "o_orderdate"], n),
+                 lambda r: _between(r.c("o_orderdate"), "1995-01-01", "1996-12-31"))
+    cu = _tpch_scan("customer", ["c_custkey", "c_nationkey"], n)
+    n1 = _tpch_scan("nation", ["n_nationkey", "n_regionkey"], n)
+    n2 = _tpch_scan("nation", ["n_nationkey", "n_name"], n)
+    re = _filter(_tpch_scan("region", ["r_regionkey", "r_name"], n), lambda r: binary(r.c("r_name"), "Eq", literal("Utf8", "AMERICA")))
+    j = _join(su, li, [("s_suppkey", "l_suppkey")], n)
+    j = _join(j, pt, [("l_partkey", "p_partkey")], n)
+    j = _join(j, od, [("l_orderkey", "o_orderkey")], n)
+    j = _join(j, cu, [("o_custkey", "c_custkey")], n)
+    j = _join(j, n1, [("c_nationkey", "n_nationkey")], n)
+    j = _join(j, n2, [("s_nationkey", "n_nationkey")], n)
+    j = _join(j, re, [("n_regionkey", "r_regionkey")], n)
+    nations = _subquery(j, [(date_part("YEAR", j.c("o_orderdate")), "o_year"), (_revenue(j), "volume"), (j.c("n_name"), "nation")])
+    brazil = case_expr([(binary(nations.c("nation"), "Eq", literal("Utf8", "BRAZIL")), nations.c("volume"))], _f64(0))
+    aggrs = [_sum("SUM(CASE WHEN all_nations.nation = Utf8(\"BRAZIL\") THEN all_nations.volume ELSE Int64(0) END)", brazil),
+             _sum("SUM(all_nations.volume)", nations.c("volume"))]
+    g = _grouped(nations, ["o_year"], aggrs, n)
+    share = binary(g.c(aggrs[0]["name"]), "Divide", g.c(aggrs[1]["name"]))
+    return _project_sort(g, [(g.c("o_year"), "o_year"), (share, "mkt_share")], [("o_year", False)])
+
+
+def tpch_q9(n: int = TARGET_PARTITIONS) -> dict:
+    su = _tpch_scan("supplier", ["s_suppkey", "s_nationkey"], n)
+    li = _tpch_scan("lineitem", ["l_orderkey", "l_partkey", "l_suppkey", "l_quantity", "l_extendedprice", "l_discount"], n)
+    pt = _filter(_tpch_scan("part", ["p_partkey", "p_name"], n), lambda r: binary(r.c("p_name"), "Like", literal("Utf8", "%green%")))
+    ps = _tpch_scan("partsupp", ["ps_partkey", "ps_suppkey", "ps_supplycost"], n)
+    od = _tpch_scan("orders", ["o_orderkey", "o_orderdate"], n)
+    na = _tpch_scan("nation", ["n_nationkey", "n_name"], n)
+    j = _join(su, li, [("s_suppkey", "l_suppkey")], n)
+    j = _join(j, pt, [("l_partkey", "p_partkey")], n)
+    j = _join(j, ps, [("l_suppkey", "ps_suppkey"), ("l_partkey", "ps_partkey")], n)
+    j = _join(j, od, [("l_orderkey", "o_orderkey")], n)
+    j = _join(j, na, [("s_nationkey", "n_nationkey")], n)
+    amount = binary(_revenue(j), "Minus", binary(j.c("ps_supplycost"), "Multiply", j.c("l_quantity")))
+    profit = _subquery(j, [(j.c("n_name"), "nation"), (date_part("YEAR", j.c("o_orderdate")), "o_year"), (amount, "amount")])
+    total = _sum("SUM(profit.amount)", profit.c("amount"))
+    g = _grouped(profit, ["nation", "o_year"], [total], n)
+    return _project_sort(g, [(g.c("nation"), "nation"), (g.c("o_year"), "o_year"), (g.c(total["name"]), "sum_profit")],
+                         [("nation", False), ("o_year", True)])
+
+
+# q7 / q8 / q9: kept apart from TPCH_QUERIES, whose every entry the existing suites iterate and run through sqlite3,
+# which has no EXTRACT.  nation is scanned twice by q7 and q8, and each scan is fed its own copy.
+TPCH_MORE_QUERIES = {"q7": tpch_q7, "q8": tpch_q8, "q9": tpch_q9}
+TPCH_MORE_SOURCES = {"q7": ["supplier", "lineitem", "orders", "customer", "nation", "nation"],
+                     "q8": ["supplier", "lineitem", "part", "orders", "customer", "nation", "nation", "region"],
+                     "q9": ["supplier", "lineitem", "part", "partsupp", "orders", "nation"]}

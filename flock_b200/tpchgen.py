@@ -1,15 +1,15 @@
 """TPC-H tables in Flock's schemas (flock/src/datasource/tpch/mod.rs), generated from a seed with vectorised numpy.
 
-The value rules are those of the TPC-H specification, section 4.2.3, wherever the predicates of q1, q3, q5, q6, q10,
+The value rules are those of the TPC-H specification, section 4.2.3, wherever the predicates of q1, q3, q5 to q10,
 q12 and q14 can see them: cardinalities per scale factor, sparse order keys (the first 8 of every 32), customer keys
 never divisible by 3, the date ranges (STARTDATE 1992-01-01, CURRENTDATE 1995-06-17, ENDDATE 1998-12-31) with the
 ship, commit and receipt offsets, return flag and line status against CURRENTDATE, the quantity, discount and tax
 ranges, P_RETAILPRICE's formula, L_EXTENDEDPRICE = L_QUANTITY * P_RETAILPRICE, L_SUPPKEY from the part's four
 partsupp suppliers, the segment, priority, ship mode, ship instruction, P_TYPE syllable, container and brand lists, the
-fixed 25 nations and 5 regions, and O_TOTALPRICE / O_ORDERSTATUS derived from the order's lines.  Money is integer
-cents divided by 100.  Comments, names, addresses and phone digits come from a small vocabulary instead of the
-specification's text grammar (no query here reads them except as opaque group keys).  Dates are Date32: days since
-1970-01-01.
+fixed 25 nations and 5 regions, P_NAME's five distinct colour words, and O_TOTALPRICE / O_ORDERSTATUS derived from the
+order's lines.  Money is integer cents divided by 100.  Comments, addresses and phone digits come from a small
+vocabulary instead of the specification's text grammar (no query here reads them except as opaque group keys).  Dates
+are Date32: days since 1970-01-01.
 """
 from __future__ import annotations
 
@@ -32,8 +32,13 @@ TYPE_S2 = ["ANODIZED", "BURNISHED", "PLATED", "POLISHED", "BRUSHED"]
 TYPE_S3 = ["TIN", "NICKEL", "BRASS", "STEEL", "COPPER"]
 CONTAINER_S1 = ["SM", "LG", "MED", "JUMBO", "WRAP"]
 CONTAINER_S2 = ["CASE", "BOX", "BAG", "JAR", "PKG", "PACK", "CAN", "DRUM"]
-COLORS = ["almond", "antique", "aquamarine", "azure", "beige", "bisque", "black", "blanched", "blue", "blush", "brown", "burlywood",
-          "chartreuse", "chiffon", "chocolate", "coral", "cornflower", "cornsilk", "cream", "cyan", "dark", "deep", "dim", "dodger"]
+# P_NAME's words (the specification's 4.2.3 colour list)
+COLORS = ("almond antique aquamarine azure beige bisque black blanched blue blush brown burlywood burnished chartreuse chiffon "
+          "chocolate coral cornflower cornsilk cream cyan dark deep dim dodger drab firebrick floral forest frosted gainsboro ghost "
+          "goldenrod green grey honeydew hot indian ivory khaki lace lavender lawn lemon light lime linen magenta maroon medium "
+          "metallic midnight mint misty moccasin navajo navy olive orange orchid pale papaya peach peru pink plum powder puff purple "
+          "red rose rosy royal saddle salmon sandy seashell sienna sky slate smoke snow spring steel tan thistle tomato turquoise "
+          "violet wheat white yellow").split()
 WORDS = ["furiously", "carefully", "quickly", "slyly", "blithely", "final", "regular", "special", "pending", "express", "ironic",
          "bold", "even", "silent", "unusual", "deposits", "requests", "accounts", "packages", "theodolites", "instructions", "foxes"]
 
@@ -101,6 +106,23 @@ def order_keys(n: int) -> np.ndarray:
     return (i // 8) * 32 + (i % 8) + 1
 
 
+def part_names(seed: int, n: int) -> np.ndarray:
+    """P_NAME: five distinct words of COLORS, drawn from a generator derived from `seed`."""
+    rng = np.random.default_rng([seed, 1])
+    words = rng.integers(0, len(COLORS), (n, 5))
+    while True:
+        s = np.sort(words, axis=1)
+        dup = np.any(s[:, 1:] == s[:, :-1], axis=1)
+        if not dup.any():
+            break
+        words[dup] = rng.integers(0, len(COLORS), (int(dup.sum()), 5))
+    w = np.array(COLORS)[words]
+    out = w[:, 0]
+    for k in range(1, 5):
+        out = np.char.add(np.char.add(out, " "), w[:, k])
+    return out
+
+
 def generate(scale: float = 0.01, seed: int = 42, columns: dict[str, list[str]] | None = None) -> dict[str, pa.Table]:
     """All eight tables (or, with `columns`, only the listed tables and columns) at scale factor `scale`."""
     rng = np.random.default_rng(seed)
@@ -117,7 +139,11 @@ def generate(scale: float = 0.01, seed: int = 42, columns: dict[str, list[str]] 
     types = np.char.add(np.char.add(np.char.add(np.char.add(np.array(TYPE_S1)[t1], " "), np.array(TYPE_S2)[t2]), " "), np.array(TYPE_S3)[t3])
     m, b = rng.integers(1, 6, P), rng.integers(1, 6, P)
     containers = np.char.add(np.char.add(np.array(CONTAINER_S1)[rng.integers(0, 5, P)], " "), np.array(CONTAINER_S2)[rng.integers(0, 8, P)])
-    names = np.char.add(np.char.add(np.array(COLORS)[rng.integers(0, len(COLORS), P)], " "), np.array(COLORS)[rng.integers(0, len(COLORS), P)])
+    # Names once took two words of 24 from this stream.  Those draws stay, unused, so that every other column keeps its
+    # values for a seed; the names come from a generator of their own.
+    rng.integers(0, 24, P)
+    rng.integers(0, 24, P)
+    names = part_names(seed, P)
     p_price_cents = retailprice_cents(pk)
     out["part"] = {"p_partkey": pa.array(pk), "p_name": pa.array(names.astype(object), _S),
                    "p_mfgr": pa.array(np.char.add("Manufacturer#", m.astype(str)).astype(object), _S),

@@ -282,10 +282,17 @@ enum flockgpu_op {
   /* x [NOT] LIKE pattern: pops, in push order, x (Utf8) and the pattern (a LIT_UTF8, or LIT_NULL).  Case-sensitive; '%'
    * matches any run of characters, '_' exactly one UTF-8 code point; there is no escape character.  NULL in, NULL out. */
   FLOCKGPU_OP_LIKE = 46,
-  FLOCKGPU_OP_NOT_LIKE = 47
+  FLOCKGPU_OP_NOT_LIKE = 47,
+  /* date_part(field, x), SQL's EXTRACT(field FROM x): pops x, a Date32 or a Timestamp without a timezone (any unit);
+   * `col` = FLOCKGPU_DATE_PART_*.  The result is Int32: YEAR is the proleptic Gregorian year of the day holding x
+   * (year 0 exists), NULL only where it does not fit Int32; HOUR is the hour of that day (0 for a Date32).  NULL in,
+   * NULL out.                                                                                                          */
+  FLOCKGPU_OP_DATE_PART = 48
 };
 #define FLOCKGPU_CASE_HAS_BASE 1
 #define FLOCKGPU_CASE_HAS_ELSE 2
+#define FLOCKGPU_DATE_PART_YEAR 1
+#define FLOCKGPU_DATE_PART_HOUR 2
 typedef struct flockgpu_expr_token {
   int32_t op;      /* enum flockgpu_op                                      */
   int32_t dtype;   /* enum flockgpu_dtype: CAST target / literal type       */
