@@ -129,15 +129,6 @@ __global__ void __launch_bounds__(DC_THREADS, DC_MIN_CTAS) dim_count_kernel(cons
 }
 
 // ------------------------------------------------------------------------------------------------
-static ColRef colref_of(const Column& c) {
-  ColRef r{};
-  r.data = c.values();
-  r.offsets = c.offs();
-  r.dtype = c.dtype;
-  r.validity = c.valid();
-  return r;
-}
-
 bool dim_count_key_type(int dtype) {
   return dtype == FLOCKGPU_INT32 || dtype == FLOCKGPU_DATE32 || dtype == FLOCKGPU_INT64 || dtype == FLOCKGPU_UINT64 || dtype == FLOCKGPU_TIMESTAMP || dtype == FLOCKGPU_UTF8;
 }
@@ -187,13 +178,11 @@ TablePtr dim_count_aggregate(const CtxPtr& ctx, const TablePtr& fact_ptr, int fa
     a.fact_key.col[0] = fact_key;
     a.dim_key = b.key;
     a.dim_cols[0] = b.cols[0];
-    for (size_t i = 0; i < fact.cols.size(); ++i) a.fact_cols[i] = colref_of(fact.cols[i]);
+    fill_colrefs(fact, a.fact_cols);
     if (predicate) {
-      std::vector<ColInfo> infos;
-      for (const Column& c : fact.cols) infos.push_back({c.dtype, c.name, c.format, c.validity != nullptr});
-      CompiledPredicate cp = compile_predicate(*predicate, infos);
+      CompiledPredicate cp = compile_predicate(*predicate, col_infos(fact));
+      // the kernel never reports a division by zero
       FG_CHECK(!cp.prog.has_div_by_col, FLOCKGPU_ERR_INVALID, "dim_count: a predicate that divides by a column stays in its own filter");
-      FG_CHECK(!cp.lossy_cast, FLOCKGPU_ERR_INVALID, "dim_count: a predicate with a CAST that can give NULL stays in its own filter");
       a.has_pred = 1;
       a.pred = cp.prog;
     }

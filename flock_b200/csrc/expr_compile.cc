@@ -59,8 +59,8 @@ int promote(int a, int b) {
 
 // A CAST from `from` to `to` that some source value does not survive (cast_fits): Float64 to an integer type, an
 // integer type to a narrower one or across signedness.  The tree form gives NULL for the values that do not fit.  The
-// chain form has no NULLs of its own: it lowers an explicit one as a plain conversion and flags it (`lossy_cast` of
-// CompiledValue / CompiledPredicate), and the operators evaluate a flagged expression in the tree form.
+// chain form has no NULLs of its own: compile_value and compile_predicate refuse an expression that holds one, and the
+// operators evaluate it in the tree form.
 bool lossy_cast(int from, int to) {
   if (from == to || to == FLOCKGPU_FLOAT64) return false;
   if (from == FLOCKGPU_FLOAT64) return true;
@@ -72,6 +72,12 @@ struct Tree {
   std::vector<Node> nodes;
   int root = -1;
 };
+
+bool has_lossy_cast(const Tree& t) {
+  for (const Node& n : t.nodes)
+    if (n.op == FLOCKGPU_OP_CAST && lossy_cast(t.nodes[n.l].dtype, n.dtype)) return true;
+  return false;
+}
 
 // The unit of date_part's Timestamp operand `idx`: that of the first Timestamp column it reads, as compile_value keeps
 // the format of a computed Timestamp.  A timezone, or no Timestamp column at all (a literal), is refused.
@@ -283,7 +289,6 @@ Val literal_as(const Node& n, int dtype) {
 struct ChainBuilder {
   const Tree& t;
   bool div_by_col = false;
-  bool lossy = false;  // an explicit CAST that can lose its value, lowered without its NULLs
   explicit ChainBuilder(const Tree& tree) : t(tree) {}
 
   static void push(Chain& c, ChainStep st) {
@@ -397,7 +402,6 @@ struct ChainBuilder {
       return c;
     }
     if (n.op == FLOCKGPU_OP_CAST) {
-      lossy |= lossy_cast(t.nodes[n.l].dtype, n.dtype);
       c = build(n.l);
       convert(c, t.nodes[n.l].dtype, n.dtype);
       return c;
@@ -485,7 +489,7 @@ int infer_dtype(const Expr& e, const std::vector<ColInfo>& cols) {
   return t.nodes[t.root].dtype;
 }
 
-CompiledValue compile_value(const Expr& e, const std::vector<ColInfo>& cols) {
+CompiledValue compile_value(const Expr& e, const std::vector<ColInfo>& cols, int max_null_inputs) {
   Tree t = build_tree(e, cols);
   const Node& root = t.nodes[t.root];
   CompiledValue out;
@@ -501,7 +505,17 @@ CompiledValue compile_value(const Expr& e, const std::vector<ColInfo>& cols) {
   ChainBuilder b(t);
   out.chain = b.build(t.root);
   out.has_div_by_col = b.div_by_col;
-  out.lossy_cast = b.lossy;
+  auto note = [&](int col) {
+    if (col >= 0 && cols[col].has_nulls) out.null_inputs.push_back(col);
+  };
+  note(out.chain.start_col);
+  for (int st = 0; st < out.chain.n_steps; ++st)
+    if (out.chain.steps[st].src == 1) note(out.chain.steps[st].col);
+  FG_CHECK(int(out.null_inputs.size()) <= max_null_inputs, FLOCKGPU_ERR_UNSUPPORTED, "projection: more than %d inputs with NULLs for the chain form",
+           max_null_inputs);
+  // a NULL operand makes the quotient NULL, whatever value sits under it: the chain divides it all the same
+  FG_CHECK(!out.has_div_by_col || out.null_inputs.empty(), FLOCKGPU_ERR_UNSUPPORTED, "projection: a division by a column over columns with NULLs");
+  FG_CHECK(!has_lossy_cast(t), FLOCKGPU_ERR_UNSUPPORTED, "projection: a CAST that can give NULL");
   out.format = default_format(root.dtype);
   if (root.dtype == FLOCKGPU_TIMESTAMP) {
     // keep the unit/timezone of the first timestamp column the expression touches
@@ -598,7 +612,7 @@ CompiledPredicate compile_predicate(const Expr& e, const std::vector<ColInfo>& c
   };
   collect(t.root);
   p.has_div_by_col = b.div_by_col ? 1 : 0;
-  out.lossy_cast = b.lossy;
+  FG_CHECK(!has_lossy_cast(t), FLOCKGPU_ERR_UNSUPPORTED, "filter: a CAST that can give NULL");
   bool any_null = false;
   for (int i = 0; i < p.n_terms; ++i) any_null |= p.terms[i].null_cols != 0;
 
@@ -616,6 +630,8 @@ CompiledPredicate compile_predicate(const Expr& e, const std::vector<ColInfo>& c
   } else {
     // SQL three-valued logic (strong Kleene): 1 = TRUE, 0 = FALSE, 2 = NULL; the row is kept iff the root is TRUE
     FG_CHECK(p.n_terms <= 4, FLOCKGPU_ERR_UNSUPPORTED, "filter: more than 4 comparison terms over columns with NULLs");
+    // the terms divide in the rows where an operand is NULL too
+    FG_CHECK(!p.has_div_by_col, FLOCKGPU_ERR_UNSUPPORTED, "filter: a division by a column over columns with NULLs");
     p.kleene = 1;
     std::function<int(int, unsigned)> k3 = [&](int idx, unsigned bits) -> int {
       const Node& n = t.nodes[idx];

@@ -35,7 +35,6 @@ struct FastPred {
 struct CompiledPredicate {
   Predicate prog;
   FastPred fast;
-  bool lossy_cast = false;  // holds a CAST that can give NULL, lowered without it: the operators take the tree form
 };
 
 enum FastValueKind {
@@ -49,7 +48,7 @@ struct CompiledValue {
   int dtype = FLOCKGPU_INT64;
   std::string format;  // Arrow format of the result
   bool has_div_by_col = false;
-  bool lossy_cast = false;  // holds a CAST that can give NULL, lowered without it: the operators take the tree form
+  std::vector<int> null_inputs;  // the columns with NULLs the chain reads, once per read: the value is NULL where one is
   int fast = FAST_VAL_NONE;
   double fast_lit = 0;
 };
@@ -76,13 +75,21 @@ struct CompiledTree {
 CompiledTree compile_tree_values(const std::vector<Expr>& exprs, const std::vector<ColInfo>& cols);
 CompiledTree compile_tree_predicate(const Expr& e, const std::vector<ColInfo>& cols);
 
-// ColInfo / ColRef views of a table's columns (filter_project.cu)
+// ColInfo / ColRef views of a table's columns (filter_project.cu); filter_colrefs refuses more than MAX_IN_COLS columns
+// and a column that is NULL as a whole.
 std::vector<ColInfo> col_infos(const Table& t);
-void fill_colrefs(const Table& t, ColRef* refs);
+void filter_colrefs(const Table& t, ColRef* refs);
 
+// A value in the chain form is NULL where a column it reads is: a pure projection ANDs the validity of at most this many
+// reads (and_validity_kernel).  The fused filter kernel writes no validity, so a value computed there reads none.
+constexpr int PROJECT_MAX_NULL_INPUTS = 4;
+
+// The term and chain forms.  Both fail with FLOCKGPU_ERR_UNSUPPORTED, naming the reason, on what they cannot evaluate
+// exactly, and the operators then take the tree form: a CAST that can give NULL, a division by a column over columns
+// with NULLs, and in compile_value more than `max_null_inputs` reads of columns with NULLs (a plain column passes).
 Expr tokens_to_expr(const flockgpu_expr* e);
 CompiledPredicate compile_predicate(const Expr& e, const std::vector<ColInfo>& cols);
-CompiledValue compile_value(const Expr& e, const std::vector<ColInfo>& cols);
+CompiledValue compile_value(const Expr& e, const std::vector<ColInfo>& cols, int max_null_inputs);
 // Result type of a value expression without building the chain (used for output schemas).
 int infer_dtype(const Expr& e, const std::vector<ColInfo>& cols);
 std::string expr_to_string(const Expr& e, const std::vector<ColInfo>& cols);

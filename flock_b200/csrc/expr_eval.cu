@@ -51,7 +51,7 @@ std::vector<Column> eval_exprs(const CtxPtr& ctx, const Table& in, const std::ve
   args->n_rows = in.num_rows;
   args->err_flag = reinterpret_cast<int*>(ctx->d_scalars + 8);
   args->prog = ct.prog;
-  fill_colrefs(in, args->cols);
+  filter_colrefs(in, args->cols);
   std::vector<Column> out;
   for (size_t i = 0; i < exprs.size(); ++i) {
     const TreeRoot& r = ct.roots[i];

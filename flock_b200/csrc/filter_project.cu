@@ -522,17 +522,25 @@ std::vector<ColInfo> col_infos(const Table& t) {
   return v;
 }
 
+ColRef colref_of(const Column& c) {
+  ColRef r{};
+  r.data = c.values();
+  r.offsets = c.offs();
+  r.dtype = c.dtype;
+  r.chunk_shift = c.chunks ? c.chunks->shift : 0;
+  r.chunks = c.chunks ? static_cast<const void* const*>(c.chunks->table->ptr) : nullptr;
+  r.validity = c.valid();
+  return r;
+}
+
 void fill_colrefs(const Table& t, ColRef* refs) {
+  for (size_t i = 0; i < t.cols.size(); ++i) refs[i] = colref_of(t.cols[i]);
+}
+
+void filter_colrefs(const Table& t, ColRef* refs) {
   FG_CHECK(t.cols.size() <= size_t(MAX_IN_COLS), FLOCKGPU_ERR_UNSUPPORTED, "filter_project: more than %d input columns", MAX_IN_COLS);
-  for (size_t i = 0; i < t.cols.size(); ++i) {
-    FG_CHECK(!t.cols[i].all_null, FLOCKGPU_ERR_UNSUPPORTED, "filter_project: NULL input column \"%s\"", t.cols[i].name.c_str());
-    refs[i].data = t.cols[i].values();
-    refs[i].offsets = t.cols[i].offs();
-    refs[i].dtype = t.cols[i].dtype;
-    refs[i].chunk_shift = t.cols[i].chunks ? t.cols[i].chunks->shift : 0;
-    refs[i].chunks = t.cols[i].chunks ? static_cast<const void* const*>(t.cols[i].chunks->table->ptr) : nullptr;
-    refs[i].validity = t.cols[i].valid();
-  }
+  for (const Column& c : t.cols) FG_CHECK(!c.all_null, FLOCKGPU_ERR_UNSUPPORTED, "filter_project: NULL input column \"%s\"", c.name.c_str());
+  fill_colrefs(t, refs);
 }
 
 // Launches the filter over the whole relation in tiles of FP_THREADS x PredFn::I rows.  The grid is the resident CTAs
@@ -601,7 +609,7 @@ TablePtr filter_project(const CtxPtr& ctx, const TablePtr& in_ptr, const Expr* p
     for (size_t i = 0; i < projections.size() && plain; ++i) {
       CompiledValue v;
       try {
-        v = compile_value(projections[i], dinfos);
+        v = compile_value(projections[i], dinfos, PROJECT_MAX_NULL_INPUTS);
       } catch (const Error& err) {
         if (err.code != FLOCKGPU_ERR_UNSUPPORTED) throw;  // not a plain column: compiled again, for the tree form, below
       }
@@ -633,18 +641,7 @@ TablePtr filter_project(const CtxPtr& ctx, const TablePtr& in_ptr, const Expr* p
     bool tree = false;
     for (const Expr& e : projections) {
       try {
-        CompiledValue v = compile_value(e, infos);
-        // the chain kernels read at most 4 validity inputs, and none inside the fused filter
-        int null_inputs = 0;
-        auto note = [&](int col) { null_inputs += col >= 0 && in.cols[col].validity; };
-        note(v.chain.start_col);
-        for (int st = 0; st < v.chain.n_steps; ++st)
-          if (v.chain.steps[st].src == 1) note(v.chain.steps[st].col);
-        if (!v.passthrough && null_inputs > (predicate ? 0 : 4)) fail(FLOCKGPU_ERR_UNSUPPORTED, "projection: more NULL inputs than the chain form carries");
-        // a NULL operand makes the quotient NULL, whatever value sits under it: the chain form divides it all the same
-        if (v.has_div_by_col && null_inputs > 0) fail(FLOCKGPU_ERR_UNSUPPORTED, "projection: a division over columns with NULLs");
-        if (v.lossy_cast) fail(FLOCKGPU_ERR_UNSUPPORTED, "projection: a CAST that can give NULL");
-        vals.push_back(v);
+        vals.push_back(compile_value(e, infos, predicate ? 0 : PROJECT_MAX_NULL_INPUTS));
         tree_vals.push_back(false);
       } catch (const Error& err) {
         if (err.code != FLOCKGPU_ERR_UNSUPPORTED) throw;
@@ -697,7 +694,7 @@ TablePtr filter_project(const CtxPtr& ctx, const TablePtr& in_ptr, const Expr* p
     ProjectArgs pa{};
     pa.n_rows = in.num_rows;
     pa.err_flag = err_flag;
-    fill_colrefs(in, pa.cols);
+    filter_colrefs(in, pa.cols);
     for (size_t i = 0; i < vals.size(); ++i) {
       const CompiledValue& v = vals[i];
       Column c;
@@ -718,14 +715,8 @@ TablePtr filter_project(const CtxPtr& ctx, const TablePtr& in_ptr, const Expr* p
       } else {
         // a computed value is NULL where any column it reads is NULL
         std::vector<const uint8_t*> srcs;
-        auto note = [&](int col) {
-          if (col >= 0 && in.cols[col].validity) srcs.push_back(in.cols[col].valid());
-        };
-        note(v.chain.start_col);
-        for (int st = 0; st < v.chain.n_steps; ++st)
-          if (v.chain.steps[st].src == 1) note(v.chain.steps[st].col);
+        for (int col : v.null_inputs) srcs.push_back(in.cols[col].valid());
         if (!srcs.empty() && in.num_rows > 0) {
-          FG_CHECK(srcs.size() <= 4, FLOCKGPU_ERR_UNSUPPORTED, "projection: an expression over more than 4 columns with NULLs");
           c.validity = alloc(ctx, size_t(in.num_rows));
           c.nullable = true;
           int grid = int(std::min<int64_t>((in.num_rows + 255) / 256, int64_t(ctx->sm_count) * 8));
@@ -804,9 +795,6 @@ TablePtr filter_project(const CtxPtr& ctx, const TablePtr& in_ptr, const Expr* p
   bool use_tree = false;
   try {
     cp = compile_predicate(*predicate, infos);
-    // the term form divides in the rows where an operand is NULL too (kleene: a referenced column has NULLs)
-    if (cp.prog.has_div_by_col && cp.prog.kleene) fail(FLOCKGPU_ERR_UNSUPPORTED, "filter: a division over columns with NULLs");
-    if (cp.lossy_cast) fail(FLOCKGPU_ERR_UNSUPPORTED, "filter: a CAST that can give NULL");
   } catch (const Error& err) {
     if (err.code != FLOCKGPU_ERR_UNSUPPORTED) throw;
     tree_pred = compile_tree_predicate(*predicate, infos);
@@ -845,7 +833,7 @@ TablePtr filter_project(const CtxPtr& ctx, const TablePtr& in_ptr, const Expr* p
   fa.n_rows = in.num_rows;
   fa.out_count = ctx->d_scalars + 0;
   fa.err_flag = err_flag;
-  fill_colrefs(in, fa.cols);
+  filter_colrefs(in, fa.cols);
   // What a launch that starts before the kernel ahead of it completes reads early (compact.cuh: EarlyStart): the
   // relation's device-resident buffers, all older than the outputs allocated below.
   EarlyStart early{0, ++ctx->alloc_seq};
@@ -865,15 +853,6 @@ TablePtr filter_project(const CtxPtr& ctx, const TablePtr& in_ptr, const Expr* p
     c.dtype = v.dtype;
     c.format = v.format;
     if (v.passthrough) c.nullable = in.cols[v.src_col].nullable;
-    if (!v.passthrough) {
-      // a computed output inside the fused filter kernel cannot carry NULLs (no validity output there)
-      auto refuse = [&](int col) {
-        if (col >= 0) require_no_nulls(in.cols[col], "filter: computed projection");
-      };
-      refuse(v.chain.start_col);
-      for (int st = 0; st < v.chain.n_steps; ++st)
-        if (v.chain.steps[st].src == 1) refuse(v.chain.steps[st].col);
-    }
     if (v.dtype == FLOCKGPU_UTF8 || (v.passthrough && in.cols[v.src_col].validity)) {
       // Utf8 outputs and outputs with validity bytes are taken through the selection vector behind the kernel
       need_sel = true;
@@ -991,7 +970,7 @@ TablePtr select_group_match_rows(const CtxPtr& ctx, const Table& in, int key_col
   fa.n_rows = in.num_rows;
   fa.out_count = ctx->d_scalars + 0;
   fa.err_flag = reinterpret_cast<int*>(ctx->d_scalars + 8);
-  fill_colrefs(in, fa.cols);
+  filter_colrefs(in, fa.cols);
   auto out = std::make_shared<Table>();
   out->ctx = ctx;
   out->metadata = in.metadata;

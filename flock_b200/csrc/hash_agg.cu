@@ -1626,14 +1626,7 @@ AggPlan plan_aggregates(const Table& in, int mode, const std::vector<AggSpec>& a
 
 void fill_cols(const Table& t, ColRef* refs) {
   FG_CHECK(t.cols.size() <= size_t(MAX_IN_COLS), FLOCKGPU_ERR_UNSUPPORTED, "hash_aggregate: more than %d input columns", MAX_IN_COLS);
-  for (size_t i = 0; i < t.cols.size(); ++i) {
-    refs[i].data = t.cols[i].values();
-    refs[i].offsets = t.cols[i].offs();
-    refs[i].dtype = t.cols[i].dtype;
-    refs[i].chunk_shift = 0;
-    refs[i].chunks = nullptr;
-    refs[i].validity = t.cols[i].valid();
-  }
+  fill_colrefs(t, refs);
 }
 
 int grid_for(const CtxPtr& ctx, int64_t items, int threads, int per_sm) {

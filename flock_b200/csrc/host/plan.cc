@@ -753,20 +753,16 @@ static JoinCount join_count(const ExecEnv& env, const HashAggregateExec& agg, co
   if (in[dim]->num_rows > fg::DIM_COUNT_MAX_ROWS) return generic();
   Expr pred;
   if (filter[fact]) {
+    // dim_count interprets the term form, and reports no division by zero: any other predicate runs as its own filter
+    // first, which takes the tree form where the term form refuses it
     emit_expr(*filter[fact]->predicate, *in[fact], &pred);
-    // dim_count interprets the term form, which has no date_part: such a predicate runs as its own filter first
-    if (std::any_of(pred.begin(), pred.end(), [](const ExprTok& t) { return t.op == FLOCKGPU_OP_DATE_PART; })) {
-      in[fact] = filter[fact]->apply(env, in[fact]);
-      filter[fact] = nullptr;
-      pred.clear();
+    bool term_form = false;
+    try {
+      term_form = !fg::compile_predicate(pred, fg::col_infos(*in[fact])).prog.has_div_by_col;
+    } catch (const fg::Error& err) {
+      if (err.code != FLOCKGPU_ERR_UNSUPPORTED) throw;
     }
-  }
-  if (filter[fact]) {
-    std::vector<fg::ColInfo> infos;
-    for (const fg::Column& c : in[fact]->cols) infos.push_back({c.dtype, c.name, c.format, c.validity != nullptr});
-    // the filter reports a division by zero itself, and evaluates a CAST that can give NULL in the tree form
-    const fg::CompiledPredicate cp = fg::compile_predicate(pred, infos);
-    if (cp.prog.has_div_by_col || cp.lossy_cast) {
+    if (!term_form) {
       in[fact] = filter[fact]->apply(env, in[fact]);
       filter[fact] = nullptr;
     }

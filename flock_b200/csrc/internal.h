@@ -441,6 +441,12 @@ inline void require_no_nulls(const Column& c, const char* what) {
   if (c.validity) fail(FLOCKGPU_ERR_UNSUPPORTED, "%s: column \"%s\" contains NULLs, which this operator does not handle on the GPU path", what, c.name.c_str());
 }
 
+// The kernels' view of a column (expr_program.h); fill_colrefs writes refs[i] for every column i of `t`, and each caller
+// checks first that they fit its argument block (filter_project.cu).
+struct ColRef;
+ColRef colref_of(const Column& c);
+void fill_colrefs(const Table& t, ColRef* refs);
+
 // ---- operators (implemented in the .cu files; called by the ABI layer and by the plan layer) ----
 struct ExprTok {
   int op, dtype, col;

@@ -545,17 +545,6 @@ std::vector<int> routing_columns(const Table& in, const std::vector<int>& keys) 
   return fixed.empty() ? keys : fixed;
 }
 
-static void fill_colrefs(const Table& in, ColRef* refs) {
-  for (size_t i = 0; i < in.cols.size(); ++i) {
-    refs[i].data = in.cols[i].values();
-    refs[i].offsets = in.cols[i].offs();
-    refs[i].dtype = in.cols[i].dtype;
-    refs[i].chunk_shift = 0;
-    refs[i].chunks = nullptr;
-    refs[i].validity = in.cols[i].valid();
-  }
-}
-
 PartPass partition_count_scan(const CtxPtr& ctx, const Table& in, const std::vector<int>& routing_cols, int n_parts, int dest_rank, int digit_col,
                               int digit_shift, bool ship_nullable) {
   FG_CHECK(n_parts >= 1 && n_parts <= PT_MAX_PARTS, FLOCKGPU_ERR_INVALID, "hash_partition: n_parts must be in [1, %d], got %d", PT_MAX_PARTS, n_parts);

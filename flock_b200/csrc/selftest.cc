@@ -83,12 +83,13 @@ int flockgpu_selftest_eval_predicate(const struct ArrowSchema* schema, const str
 }
 
 // Evaluates a value expression; `out` must hold rows * 8 bytes (4-byte types are written packed).
-// *out_dtype receives the flockgpu_dtype of the result, *out_passthrough 1 if it is a plain column.
+// *out_dtype receives the flockgpu_dtype of the result, *out_passthrough 1 if it is a plain column.  Compiled as a
+// pure projection compiles it: what this accepts, a ProjectionExec over the same columns runs in the chain form.
 int flockgpu_selftest_eval_value(const struct ArrowSchema* schema, const struct ArrowArray* batch, const flockgpu_expr* expr, void* out,
                                  int32_t* out_dtype, int32_t* out_passthrough) {
   return guarded([&] {
     HostBatch hb = view_batch(schema, batch);
-    CompiledValue cv = compile_value(tokens_to_expr(expr), hb.infos);
+    CompiledValue cv = compile_value(tokens_to_expr(expr), hb.infos, PROJECT_MAX_NULL_INPUTS);
     if (out_dtype) *out_dtype = cv.dtype;
     if (out_passthrough) *out_passthrough = cv.passthrough ? 1 : 0;
     if (cv.passthrough) return;

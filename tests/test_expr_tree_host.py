@@ -537,7 +537,8 @@ def test_common_subexpressions_are_computed_once():
 
 
 def test_old_forms_still_win():
-    """Everything the chain / term forms express keeps them: same fast kinds, same pass-through answers as before."""
+    """Everything the chain / term forms evaluate exactly keeps them: same fast kinds, same pass-through answers as
+    before.  What they cannot evaluate exactly, such as a lossy CAST, they refuse."""
     b = batch(64, seed=3, nulls=False)
     for e, fast in [(col(0).cast("int64") % 123 == 0, 1), (col(0).cast("int64") == 10, 2), (~(col(0).cast("int64") < 5), 2),
                     ((col(5) == "MAIL") | (col(5) == "SHIP"), 0), ((col(1) + 5) * 3 > col(0).cast("int64"), 0)]:
@@ -632,10 +633,10 @@ def test_edge_reference_agrees_with_arrow_compute():
                     pc.cast(w, dt)
 
 
-def test_lossy_cast_is_null_in_the_tree_form():
+def test_lossy_cast_is_null_in_the_tree_form_and_refused_by_the_chain():
     """CAST(Float64 AS an integer type) and narrowing integer CASTs: NULL where the target cannot hold the value
-    (arrow-rs's numeric cast), truncation toward zero otherwise.  The chain form lowers the same cast without its NULLs
-    (the operators evaluate such an expression in the tree form): it agrees wherever the value fits."""
+    (arrow-rs's numeric cast), truncation toward zero otherwise.  The chain and term forms have no NULLs of their own:
+    they refuse such a cast, and the operators evaluate it in the tree form."""
     f = [0.0, -0.0, math.inf, -math.inf, math.nan, NEG_NAN, 2.5, -2.5, 2147483647.9, 2147483648.0, -2147483648.9, -2147483649.0, -0.5, -1.0,
          4294967295.5, 4294967296.0, 2.0 ** 63, -2.0 ** 63, 9223372036854774784.0, 2.0 ** 64, 18446744073709549568.0, 1e308, 5e-324]
     i = [0, -1, I32_MIN, I32_MAX, I32_MAX + 1, I32_MIN - 1, (1 << 32) - 1, 1 << 32, I64_MIN, I64_MAX]
@@ -656,8 +657,10 @@ def test_lossy_cast_is_null_in_the_tree_form():
             same(vals, valid, want, dt)
             mask, _ = fb.selftest_eval_tree(b, e.is_null(), predicate=True)         # IS NULL sees the NULLs of the cast
             assert list(mask) == [w is None for w in want]
-            chain, cdt = fb.selftest_eval_value(b, e)
-            assert cdt == dt and all(int(c) == (w & ((1 << 64) - 1) if to == "uint64" else w) for c, w in zip(chain, want) if w is not None)
+            for chain_form in (lambda: fb.selftest_eval_value(b, e), lambda: fb.selftest_eval_predicate(b, e > 0)):
+                with pytest.raises(fb.FlockGpuError, match="a CAST that can give NULL") as info:
+                    chain_form()
+                assert info.value.code == _ffi.ERR_UNSUPPORTED
     # widening casts and implicit coercion keep wrapping, and keep the chain form
     v, dt = fb.selftest_eval_value(b, col(1).cast("float64") + col(2).cast("float64"))
     assert dt == F64

@@ -116,9 +116,10 @@ def raises_div0(fn):
 
 
 def chain_compiles(b, e, predicate):
-    """The chain / term form can lower `e` (when it cannot, the operators take the tree form)."""
+    """A filter or pure projection over `b` runs `e` in the term / chain form (when it cannot, the operators take the
+    tree form).  The whole of `b`: which columns have NULLs decides it."""
     try:
-        (fb.selftest_eval_predicate if predicate else fb.selftest_eval_value)(b.slice(0, 0), e)
+        (fb.selftest_eval_predicate if predicate else fb.selftest_eval_value)(b, e)
         return True
     except fb.FlockGpuError as err:
         return err.code != _ffi.ERR_UNSUPPORTED
@@ -184,8 +185,10 @@ def test_random_trees_in_every_role(gpu_ctx, seed, size):
                 assert_same_column(out.column(0), b.column(e.tokens[0][2]), e.tokens)   # a plain column passes through
                 continue
             assert_bits(*column_np(out.column(0)), res[0], res[1], e.tokens)
-            if n and not chain:
-                assert prof.get("expr_eval_kernel") == 1 and "project_generic_kernel" not in prof, prof
+            if n:
+                chain_kernels = sum(prof.get(k, 0) for k in ("project_generic_kernel", "project_i32_to_f64_mul_kernel"))
+                assert (chain_kernels == 1 and "expr_eval_kernel" not in prof) if chain else (chain_kernels == 0 and prof.get("expr_eval_kernel") == 1), \
+                    (chain, e.tokens, prof)
         if status == "ok" and res[0] is not None and not chain:
             tree_only.append((e, res))
     for k in range(0, len(tree_only), 4):
@@ -271,11 +274,12 @@ def test_chain_and_term_forms(gpu_ctx, size):
 
 
 def test_lossy_casts_take_the_tree_form(gpu_ctx):
-    """A CAST that can give NULL compiles to a chain too (without its NULLs): projections and filters must evaluate it
-    in the tree form, NULL where the target type cannot hold the value."""
+    """A CAST that can give NULL is refused by the chain and term forms, which have no NULLs of their own: projections
+    and filters evaluate it in the tree form, NULL where the target type cannot hold the value."""
     b = relation(8193, 3, 7)
     t = gpu_ctx.import_batches([b])
     for e in ((col(3) * 2.5).cast("int64"), col(3).cast("uint64") + 1, col(1).cast("int32"), col(2).cast("int64") - col(1)):
+        assert not chain_compiles(b, e, False) and not chain_compiles(b, e > 0, True), e.tokens
         (v, valid, _), = fb.selftest_eval_tree(b, [e])[0]
         assert not valid.all()                                         # some value of the edge relation does not fit
         out, prof = profiled(gpu_ctx, lambda: gpu_ctx.filter_project(t, None, [e]).to_batch())

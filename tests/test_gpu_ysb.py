@@ -1,8 +1,11 @@
 """The Yahoo Streaming Benchmark query on the GPU (`-m gpu`): through flock_context_unmarshal / feed / execute against the
 CPU oracle at three seeds, at 10 M events against numpy, stage by stage against the whole plan, from NDJSON text, and
 the corners of the one-pass join count (dim_count_kernel): duplicate and NULL keys, keys one byte apart, empty inputs,
-the dimension on either side, an Int32 key, no filter, and dimensions of D_MAX and D_MAX + 1 rows.  The kernels that
+the dimension on either side, an Int32 key, no filter, event filters the term form refuses, and dimensions of D_MAX and
+D_MAX + 1 rows.  The kernels that
 ran are read from the launch profile."""
+import collections
+
 import numpy as np
 import pyarrow as pa
 import pyarrow.compute as pc
@@ -45,11 +48,13 @@ def assert_schema(got):
 
 
 # ---- plans beside the reference's: the same query in other shapes ------------------------------------------------------
-def star_plan(dim_left: bool = False, with_filter: bool = True, n: int = 8) -> dict:
-    """ysb with the dimension on either side of the join, with or without the event filter."""
+def star_plan(dim_left: bool = False, with_filter: bool = True, n: int = 8, pred: dict | None = None) -> dict:
+    """ysb with the dimension on either side of the join, with or without the event filter (event_type = 'view', or
+    `pred` over ad_id 0 and event_type 1)."""
     scan = plans.repartition_rr(plans.memory_exec(plans.AD_EVENT, [2, 4]), n)
     if with_filter:
-        scan = plans.coalesce_batches_exec(plans.filter_exec(plans.binary(plans.column("event_type", 1), "Eq", plans.literal("Utf8", "view")), scan))
+        pred = pred or plans.binary(plans.column("event_type", 1), "Eq", plans.literal("Utf8", "view"))
+        scan = plans.coalesce_batches_exec(plans.filter_exec(pred, scan))
     events = plans.coalesce_batches_exec(plans.repartition_hash(scan, [plans.column("ad_id", 0)], n))
     camps = plans.coalesce_batches_exec(plans.repartition_hash(plans.repartition_rr(plans.memory_exec(plans.CAMPAIGN, [0, 1]), n), [plans.column("c_ad_id", 0)], n))
     if dim_left:   # c_ad_id 0, campaign_id 1, ad_id 2, event_type 3
@@ -223,6 +228,27 @@ def test_dimension_on_either_side_with_and_without_filter(gpu_ctx, dim_left, wit
     oracle.assert_tables_equal(got, want)
     if not with_filter:
         assert sum(got[COUNT].to_pylist()) == 80_000
+
+
+@pytest.mark.parametrize("kind", ["in_list", "like", "is_not_null"])
+def test_fact_filter_the_term_form_refuses_runs_first(gpu_ctx, kind):
+    """An event filter the term form cannot evaluate runs as its own filter, in the tree form, before the one-pass count."""
+    camp = ysbgen.campaigns(100, 10, 13)
+    ev = ysbgen.ad_events(100_000, camp, 13, columns=["ad_id", "event_type"])
+    etype, utf8 = plans.column("event_type", 1), lambda s: plans.literal("Utf8", s)
+    if kind == "in_list":
+        pred, keep = plans.in_list(etype, [utf8("view"), utf8("click")]), pc.is_in(ev["event_type"], value_set=pa.array(["view", "click"]))
+    elif kind == "like":
+        pred, keep = plans.binary(etype, "Like", utf8("%e%")), pc.match_like(ev["event_type"], "%e%")
+    else:
+        ev = _nullable(ev, {"event_type": np.random.default_rng(13).random(ev.num_rows) < 0.3})
+        pred, keep = plans.is_not_null(etype), pc.is_valid(ev["event_type"])
+    got, prof = run_gpu(gpu_ctx, star_plan(pred=pred), [[_split(ev, 8192)], [[camp]]])
+    kept = pa.Table.from_batches([ev]).filter(keep)
+    assert 0 < kept.num_rows < ev.num_rows
+    want = collections.Counter(kept.join(pa.Table.from_batches([camp]), "ad_id", "c_ad_id", join_type="inner")["campaign_id"].to_pylist())
+    assert dict(zip(got["campaign_id"].to_pylist(), got[COUNT].to_pylist())) == want
+    assert launches(prof, "dim_count_kernel") == 1 and all(launches(prof, k) == 0 for k in JOIN_KERNELS), sorted(prof)
 
 
 def test_int32_key_bids_by_side_input_value(gpu_ctx):

@@ -209,7 +209,7 @@ def test_three_valued_predicates_match_arrow_kleene():
         assert np.array_equal(got, want.fill_null(False).to_numpy(zero_copy_only=False)), fb.E.wrap(e).tokens
 
 
-def test_value_lowering_matches_numpy():
+def test_chain_value_lowering_matches_numpy():
     b = expr_batch(500, seed=2)
     c = cols(b)
     i32 = c["i32"]
@@ -223,8 +223,11 @@ def test_value_lowering_matches_numpy():
     assert dt == fb.FLOAT64 and np.array_equal(v.view(np.int64), (c["f64"] / 4.0 - i32.astype(np.float64)).view(np.int64))
     v, dt = fb.selftest_eval_value(b, col(4))
     assert v is None and dt == fb.TIMESTAMP                                                  # plain columns stay zero-copy
-    v, dt = fb.selftest_eval_value(b, (col(3) * 2.5).cast("int64"))
-    assert dt == fb.INT64 and np.array_equal(v, np.trunc(c["f64"] * 2.5).astype(np.int64))
+    with pytest.raises(fb.FlockGpuError, match="a CAST that can give NULL") as info:          # the chain form has no NULLs:
+        fb.selftest_eval_value(b, (col(3) * 2.5).cast("int64"))                               # the tree form evaluates it
+    assert info.value.code == _ffi.ERR_UNSUPPORTED
+    (v, valid, dt), = fb.selftest_eval_tree(b, [(col(3) * 2.5).cast("int64")])[0]
+    assert dt == fb.INT64 and valid.all() and np.array_equal(v, np.trunc(c["f64"] * 2.5).astype(np.int64))
 
 
 def test_expression_errors():
