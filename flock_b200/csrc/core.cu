@@ -89,6 +89,15 @@ std::string default_format(int dtype) {
   }
 }
 
+bool join_key_types_match(const Column& a, const Column& b) {
+  return a.dtype == b.dtype && (a.dtype != FLOCKGPU_TIMESTAMP || a.arrow_format() == b.arrow_format());
+}
+
+void check_join_key_types(const char* op, const Column& a, const Column& b) {
+  FG_CHECK(join_key_types_match(a, b), FLOCKGPU_ERR_UNSUPPORTED, "%s: key types differ (%s \"%s\" vs %s \"%s\"); DataFusion inserts casts before the join", op,
+           dtype_name(a.dtype), a.arrow_format().c_str(), dtype_name(b.dtype), b.arrow_format().c_str());
+}
+
 // ------------------------------------------------------------------------------------------------
 // context
 // ------------------------------------------------------------------------------------------------

@@ -144,8 +144,8 @@ TablePtr dim_count_aggregate(const CtxPtr& ctx, const TablePtr& fact_ptr, int fa
   FG_CHECK(fact.cols.size() <= size_t(MAX_IN_COLS), FLOCKGPU_ERR_UNSUPPORTED, "dim_count: more than %d fact columns", MAX_IN_COLS);
   const Column& fk = fact.cols[fact_key];
   const Column& dk = dim.cols[dim_key];
-  FG_CHECK(fk.dtype == dk.dtype && dim_count_key_type(fk.dtype), FLOCKGPU_ERR_UNSUPPORTED, "dim_count: key types %s / %s", dtype_name(fk.dtype),
-           dtype_name(dk.dtype));
+  check_join_key_types("dim_count", fk, dk);
+  FG_CHECK(dim_count_key_type(fk.dtype), FLOCKGPU_ERR_UNSUPPORTED, "dim_count: key type %s", dtype_name(fk.dtype));
   const int n_dim = int(dim.num_rows);
   BufferPtr counts = alloc(ctx, size_t(std::max(n_dim, 1)) * 8);
   FG_CUDA(cudaMemsetAsync(counts->ptr, 0, size_t(std::max(n_dim, 1)) * 8, ctx->stream));

@@ -2695,8 +2695,9 @@ TablePtr DeferredGroups::select_group_match(const Table& self, const int (&self_
   other.dense();
   const int ok = other_keys[kp], ov = other_keys[vp];
   if (ok < 0 || ok >= int(other.cols.size()) || ov < 0 || ov >= int(other.cols.size())) return nullptr;
-  const Column& key = core->input->cols[core->group_cols[0]];
-  if (other.cols[ok].dtype != key.dtype || other.cols[ov].dtype != o.dtype || other.cols[ok].all_null || other.cols[ov].all_null) return nullptr;
+  // hash_join has already checked both key pairs with join_key_types_match (Timestamp unit and zone included) before
+  // it asked for this selection, so the types of other's two columns are those of self's
+  if (other.cols[ok].all_null || other.cols[ov].all_null) return nullptr;
   const AggEmitArgs& ea = core->table.ea;
   GroupMatchTable gt{ea.present, ea.acc + o.a0 * ea.acc_stride, o.valid_acc >= 0 ? ea.acc + o.valid_acc * ea.acc_stride : nullptr, ea.dense_base,
                      ea.n_slots - 1};

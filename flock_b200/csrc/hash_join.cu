@@ -3,8 +3,8 @@
 // Reference operator (DataFusion fork, not in tree; used at flock/src/distributed_plan/planner.rs:169,
 // :239 and serialised in flock/src/tests/data/plan/join.json): build a hash map over ALL left batches
 // (hash -> row indices), then for every right batch emit (left_idx, right_idx) for each pair of equal
-// keys and materialise `take(left columns) ++ take(right columns)`.  NULL keys never match (no NULLs on
-// this path); duplicate keys on both sides give the full cross product.
+// keys and materialise `take(left columns) ++ take(right columns)`.  A key with a NULL or a NaN component
+// never matches; duplicate keys on both sides give the full cross product.
 //
 // GPU design: an open-addressing table with ONE slot per DISTINCT build key -- the slot holds a
 // representative build row (key equality is checked against the immutable build columns, so there is no
@@ -36,8 +36,10 @@ struct JoinSide {
   int32_t packed;
   int32_t pad;
   const void* key0;  // the key column when the join has ONE fixed-width key (kernels instantiated with KW = 4 / 8)
-  int32_t n_null_cols, pad2;  // key columns that carry validity bytes: a row with a NULL key matches nothing (NULL != NULL)
+  int32_t n_null_cols;  // key columns that carry validity bytes: a row with a NULL key matches nothing (NULL != NULL)
+  int32_t n_nan_cols;   // Float64 key columns: a row with a NaN key matches nothing (NaN != NaN)
   const uint8_t* key_valid[MAX_KEY_COLS];
+  const double* key_f64[MAX_KEY_COLS];
   KeyPack pack;
   RowKeys rk;
   ColRef cols[MAX_IN_COLS];
@@ -69,9 +71,14 @@ constexpr unsigned long long JOIN_TAG = 1ull << 63;
 // KW = 4 / 8: one fixed-width key column, read straight from JoinSide::key0 (every NEXMark join); KW = 0: the general
 // form (two packed columns, or row comparison for Utf8 / wide keys).  The general form cost ~140 lane-instructions per
 // probe row on q5 (dynamic indexing of the column table in parameter space, width and mode branches).
-__device__ __forceinline__ bool key_is_null(const JoinSide& s, int64_t row) {
+// A key with a NULL or a NaN component equals no key, its own included: such a row never enters the table and never
+// probes.  Past those two, Float64 components compare by bit pattern (-0.0 != +0.0, +inf == +inf), as DataFusion's
+// hash-then-compare does.  A join without Float64 keys has n_nan_cols = 0 and runs the NULL test alone.
+__device__ __forceinline__ bool key_matches_nothing(const JoinSide& s, int64_t row) {
   for (int i = 0; i < s.n_null_cols; ++i)
     if (!s.key_valid[i][row]) return true;
+  for (int i = 0; i < s.n_nan_cols; ++i)
+    if (isnan(s.key_f64[i][row])) return true;
   return false;
 }
 
@@ -104,7 +111,7 @@ __device__ __forceinline__ bool build_row_matches(const JoinSide& build, unsigne
 template <int KW>
 __global__ void __launch_bounds__(256) join_build_kernel(const __grid_constant__ JoinSide build, const JoinTable t) {
   for (int64_t row = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; row < build.n_rows; row += int64_t(gridDim.x) * blockDim.x) {
-    if (key_is_null(build, row)) continue;  // never enters the table: nothing can match it
+    if (key_matches_nothing(build, row)) continue;  // never enters the table: nothing can match it
     unsigned long long key;
     unsigned long long slot = side_hash<KW>(build, row, &key) & (t.cap - 1);
     if (KW == 4) {
@@ -138,7 +145,7 @@ __global__ void __launch_bounds__(256) join_build_kernel(const __grid_constant__
 template <int KW>
 __device__ __forceinline__ unsigned long long find_slot(const JoinSide& build, const JoinSide& probe, const JoinTable& t, int64_t row, unsigned* head,
                                                         unsigned* cnt) {
-  if (key_is_null(probe, row)) return ~0ull;
+  if (key_matches_nothing(probe, row)) return ~0ull;
   unsigned long long key;
   unsigned long long slot = side_hash<KW>(probe, row, &key) & (t.cap - 1);
   if (KW == 4) {
@@ -322,6 +329,7 @@ static void fill_side(const Table& t, const std::vector<int>& keys, bool packed,
   s->packed = packed ? 1 : 0;
   s->rk.n = int(keys.size());
   s->n_null_cols = 0;
+  s->n_nan_cols = 0;
   for (size_t i = 0; i < keys.size(); ++i) {
     const Column& c = t.cols[keys[i]];
     s->cols[i].data = c.values();
@@ -332,6 +340,7 @@ static void fill_side(const Table& t, const std::vector<int>& keys, bool packed,
     s->cols[i].validity = nullptr;  // key equality between the sides is value equality: rows with NULL keys are skipped up front
     s->rk.col[i] = int(i);
     if (c.validity) s->key_valid[s->n_null_cols++] = c.valid();
+    if (c.dtype == FLOCKGPU_FLOAT64) s->key_f64[s->n_nan_cols++] = static_cast<const double*>(c.values());
   }
   if (packed) {
     s->pack.n = int(keys.size());
@@ -350,6 +359,14 @@ TablePtr hash_join(const CtxPtr& ctx, const TablePtr& left_ptr, const TablePtr& 
                    const std::vector<int>& right_keys) {
   const Table& L = *left_ptr;
   const Table& R = *right_ptr;
+  // the key columns are checked before any fast path, so every path accepts and refuses the same joins
+  FG_CHECK(!left_keys.empty() && left_keys.size() == right_keys.size(), FLOCKGPU_ERR_INVALID, "hash_join: key lists must be non-empty and of equal length");
+  FG_CHECK(left_keys.size() <= size_t(MAX_KEY_COLS), FLOCKGPU_ERR_UNSUPPORTED, "hash_join: more than %d key columns", MAX_KEY_COLS);
+  for (size_t i = 0; i < left_keys.size(); ++i) {
+    const int lk = left_keys[i], rk = right_keys[i];
+    FG_CHECK(lk >= 0 && lk < int(L.cols.size()) && rk >= 0 && rk < int(R.cols.size()), FLOCKGPU_ERR_INVALID, "hash_join: key column out of range");
+    check_join_key_types("hash_join", L.cols[lk], R.cols[rk]);
+  }
   // one side is a single row and the other a group-by result still in table form (NEXMark q5: num = MAX(num)):
   // an equality selection over the table, no rows are materialised for the join
   if (left_keys.size() == 1 && right_keys.size() == 1) {
@@ -369,18 +386,8 @@ TablePtr hash_join(const CtxPtr& ctx, const TablePtr& left_ptr, const TablePtr& 
   }
   L.dense();
   R.dense();
-  FG_CHECK(!left_keys.empty() && left_keys.size() == right_keys.size(), FLOCKGPU_ERR_INVALID, "hash_join: key lists must be non-empty and of equal length");
-  FG_CHECK(left_keys.size() <= size_t(MAX_KEY_COLS), FLOCKGPU_ERR_UNSUPPORTED, "hash_join: more than %d key columns", MAX_KEY_COLS);
   std::vector<int> widths;
-  for (size_t i = 0; i < left_keys.size(); ++i) {
-    int lk = left_keys[i], rk = right_keys[i];
-    FG_CHECK(lk >= 0 && lk < int(L.cols.size()) && rk >= 0 && rk < int(R.cols.size()), FLOCKGPU_ERR_INVALID, "hash_join: key column out of range");
-    const Column& lc = L.cols[lk];
-    const Column& rc = R.cols[rk];
-    FG_CHECK(lc.dtype == rc.dtype, FLOCKGPU_ERR_UNSUPPORTED, "hash_join: key types differ (%s vs %s); DataFusion inserts casts before the join",
-             dtype_name(lc.dtype), dtype_name(rc.dtype));
-    widths.push_back(lc.width());
-  }
+  for (int lk : left_keys) widths.push_back(L.cols[lk].width());
   const bool packed = keys_packable(widths.data(), int(widths.size()));
 
   auto out = std::make_shared<Table>();
@@ -412,8 +419,9 @@ TablePtr hash_join(const CtxPtr& ctx, const TablePtr& left_ptr, const TablePtr& 
       else if (kw == 8) f(std::integral_constant<int, 8>{});
       else f(std::integral_constant<int, 0>{});
     };
-    if (kw && B.num_rows == 1 && bs.n_null_cols == 0 && ps.n_null_cols == 0) {
-      // one build row: equality filter over the probe side (see join_one_kernel)
+    if (kw && B.num_rows == 1 && bs.n_null_cols == 0 && ps.n_null_cols == 0 && ps.n_nan_cols == 0) {
+      // one build row: equality filter over the probe side (see join_one_kernel), which compares bits only -- NULL and
+      // NaN keys (a Float64 key column) take the table path, which skips them
       probe_idx = alloc(ctx, size_t(P.num_rows) * 4);
       JoinOneArgs oa{};
       oa.probe_key = ps.key0;

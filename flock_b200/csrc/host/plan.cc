@@ -741,7 +741,7 @@ static JoinCount join_count(const ExecEnv& env, const HashAggregateExec& agg, co
                       resolve_column(*in[1], join->on[0].second.name, join->on[0].second.index)};
   const fg::Column& fk = in[fact]->cols[key[fact]];
   const fg::Column& dk = in[dim]->cols[key[dim]];
-  bool ok = fk.dtype == dk.dtype && fg::dim_count_key_type(fk.dtype) && !fk.all_null && !dk.all_null && in[fact]->cols.size() <= size_t(fg::MAX_IN_COLS);
+  bool ok = fg::join_key_types_match(fk, dk) && fg::dim_count_key_type(fk.dtype) && !fk.all_null && !dk.all_null && in[fact]->cols.size() <= size_t(fg::MAX_IN_COLS);
   for (int g : group_cols) ok &= !in[dim]->cols[g].all_null;
   for (const fg::Column& c : in[fact]->cols) ok &= !c.all_null;
   if (!ok) return generic();

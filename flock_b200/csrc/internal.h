@@ -338,7 +338,15 @@ struct Column {
   const void* values() const { return data ? data->ptr : nullptr; }
   const int32_t* offs() const { return offsets ? offsets->as<int32_t>() : nullptr; }
   int width() const { return dtype_width(dtype); }
+  std::string arrow_format() const { return format.empty() ? default_format(dtype) : format; }
 };
+
+// Can a key column of one join input meet a key column of the other?  Only when both have one type: the same dtype
+// and, for a Timestamp, the same Arrow format (unit and timezone), since equal integers of unlike units are unlike
+// instants.  Date32 and Int32 are different dtypes, so they never meet.  DataFusion inserts casts before the join.
+bool join_key_types_match(const Column& a, const Column& b);
+// Fails with FLOCKGPU_ERR_UNSUPPORTED, naming both formats, when join_key_types_match(a, b) is false.
+void check_join_key_types(const char* op, const Column& a, const Column& b);
 
 struct Table;
 using TablePtr = std::shared_ptr<const Table>;

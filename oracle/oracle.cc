@@ -491,6 +491,16 @@ int64_t orc_group_by(const OCol* cols, const int32_t* keys, int n_keys, int64_t 
 }
 
 // ---- HashJoinExec (Inner) ------------------------------------------------------------------------------------
+// A key with a NaN component matches nothing, NaN itself included (DataFusion confirms hash candidates with `==`);
+// other Float64 components compare by bit pattern, so -0.0 and +0.0 do not meet.
+inline bool key_has_nan(const OCol* cols, const int32_t* keys, int n_keys, int64_t r) {
+  for (int k = 0; k < n_keys; ++k) {
+    const OCol& c = cols[keys[k]];
+    if (c.dtype == T_F64 && std::isnan(static_cast<const double*>(c.data)[r])) return true;
+  }
+  return false;
+}
+
 // Returns the number of pairs; writes up to `cap` pairs (call once with cap = 0 to size the output).
 int64_t orc_hash_join(const OCol* lcols, const int32_t* lkeys, int64_t ln, const OCol* rcols, const int32_t* rkeys, int64_t rn, int n_keys,
                       int64_t* out_left, int64_t* out_right, int64_t cap) {
@@ -498,11 +508,13 @@ int64_t orc_hash_join(const OCol* lcols, const int32_t* lkeys, int64_t ln, const
   map.reserve(size_t(ln + 16));
   std::string kb;
   for (int64_t r = 0; r < ln; ++r) {
+    if (key_has_nan(lcols, lkeys, n_keys, r)) continue;
     key_bytes(lcols, lkeys, n_keys, r, &kb);
     map[kb].push_back(r);
   }
   int64_t m = 0;
   for (int64_t r = 0; r < rn; ++r) {
+    if (key_has_nan(rcols, rkeys, n_keys, r)) continue;
     key_bytes(rcols, rkeys, n_keys, r, &kb);
     auto it = map.find(kb);
     if (it == map.end()) continue;
