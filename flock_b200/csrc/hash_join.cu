@@ -1,4 +1,4 @@
-// hash_join.cu -- K3/K4: HashJoinExec { mode: Partitioned, join_type: Inner }.
+// hash_join.cu -- K3/K4: HashJoinExec { mode: Partitioned, join_type: Inner | Semi | Anti }.
 //
 // Reference operator (DataFusion fork, not in tree; used at flock/src/distributed_plan/planner.rs:169,
 // :239 and serialised in flock/src/tests/data/plan/join.json): build a hash map over ALL left batches
@@ -18,6 +18,8 @@
 //   join_emit_kernel         second walk (table lines are L2-hot) writes the (build, probe) index pairs
 //   join_one_kernel          build side of ONE row (q5 / q7 join with a global aggregate): a stable equality
 //                            compaction over the probe side, no table
+//   semi_mark_kernel         Semi / Anti with the left side hashed: marks the slots the right rows find
+//   semi_select_kernel       Semi / Anti: stable compaction of the left rows whose key is (Semi) / is not (Anti) matched
 // and gather.cu materialises the output columns (Utf8 included).  The kernels are instantiated per key shape:
 // one 4-byte key, one 8-byte key, or the general form (two packed columns / row comparison for Utf8 keys).
 #include <algorithm>
@@ -321,6 +323,76 @@ __global__ void __launch_bounds__(256) join_emit_kernel(const __grid_constant__ 
   }
 }
 
+// ---- Semi / Anti: the left rows whose key tuple does (Semi) or does not (Anti) occur on the right, each at most once,
+// in left order.  The smaller side is hashed, as for the inner join; either way one stable compaction over the left rows
+// (compact.cuh) writes the kept rows' indices.  A row is "matched" when
+//   right side built: its key has a slot in the table;
+//   left side built:  its key's slot was marked by semi_mark_kernel (some right row probed it).  The left row finds its
+//                     slot again by a re-probe of its own key: the table lines are L2-hot, and the build kernel stays
+//                     the inner join's.
+// A left row with a NULL / NaN key component has no slot (find_slot), so it is never matched: out of Semi, in Anti.
+struct SemiMarkArgs {
+  JoinSide build, probe;  // build = the left side, probe = the right side
+  JoinTable table;
+  unsigned char* marked;  // [table.cap] 1 = a right row has the slot's key
+};
+
+template <int KW>
+__global__ void __launch_bounds__(256) semi_mark_kernel(const __grid_constant__ SemiMarkArgs a) {
+  for (int64_t row = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; row < a.probe.n_rows; row += int64_t(gridDim.x) * blockDim.x) {
+    unsigned head = 0, in_slot = 0;
+    const unsigned long long slot = find_slot<KW>(a.build, a.probe, a.table, row, &head, &in_slot);
+    if (slot != ~0ull) a.marked[slot] = 1;  // every writer stores the same value: no atomic needed
+  }
+}
+
+struct SemiSelectArgs {
+  JoinSide build, left;          // build: the hashed side (the left side itself when `marked` is set)
+  JoinTable table;
+  const unsigned char* marked;   // left side built: semi_mark_kernel's bytes; nullptr: right side built
+  int keep_matched;              // 1 Semi, 0 Anti
+  CompactScratch sc;
+  unsigned* out_idx;             // the kept left rows, ascending
+};
+
+template <int KW>
+__global__ void __launch_bounds__(CP_THREADS) semi_select_kernel(const __grid_constant__ SemiSelectArgs a) {
+  constexpr int E = 4, I = 16, G = I / E;
+  constexpr int TILE = CP_THREADS * I;
+  __shared__ CompactSmem<E, I> sm;
+  const int tid = threadIdx.x, warp = tid >> 5;
+  const int64_t n = a.left.n_rows;
+  long long tile;
+  for (int it = 0; (tile = cp_next_tile(sm, a.sc, it)) >= 0; ++it) {
+    const int64_t tile_base = tile * TILE;
+    unsigned long long bits = 0;
+#pragma unroll 1
+    for (int k = 0; k < I; ++k) {
+      const int64_t row = tile_base + cp_item_index<E>(k, tid);
+      if (row >= n) continue;
+      unsigned head = 0, in_slot = 0;
+      const unsigned long long slot = find_slot<KW>(a.build, a.left, a.table, row, &head, &in_slot);
+      const bool matched = slot != ~0ull && (!a.marked || a.marked[slot]);
+      bits |= (unsigned long long)(int(matched) == a.keep_matched) << k;
+    }
+    unsigned lane_prefix[G];
+    cp_rank_tile<E, I>(sm, a.sc, tile, bits, lane_prefix);
+    if (bits && sm.tile_total) {
+#pragma unroll
+      for (int g = 0; g < G; ++g) {
+        const unsigned nib = unsigned(bits >> (g * E)) & 0xfu;
+        if (!nib) continue;
+        const int64_t r0 = tile_base + (int64_t(g) * CP_THREADS + tid) * E;
+        const int64_t pos0 = int64_t(sm.excl) + sm.group_warp[g][warp] + lane_prefix[g];
+#pragma unroll
+        for (int e = 0; e < E; ++e)
+          if ((nib >> e) & 1u) a.out_idx[pos0 + __popc(nib & ((1u << e) - 1u))] = unsigned(r0 + e);
+      }
+    }
+    __syncthreads();
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // The kernels read the key columns only, so a side carries those alone: key i in slot i.  The other columns of the side,
 // however many, reach the output through gather_columns.
@@ -355,11 +427,8 @@ static int grid_for(const CtxPtr& ctx, int64_t items, int threads, int per_sm) {
   return int(std::max<int64_t>(1, std::min<int64_t>((items + threads - 1) / threads, int64_t(ctx->sm_count) * per_sm)));
 }
 
-TablePtr hash_join(const CtxPtr& ctx, const TablePtr& left_ptr, const TablePtr& right_ptr, const std::vector<int>& left_keys,
-                   const std::vector<int>& right_keys) {
-  const Table& L = *left_ptr;
-  const Table& R = *right_ptr;
-  // the key columns are checked before any fast path, so every path accepts and refuses the same joins
+// Every join type accepts and refuses the same key lists.
+static void check_join_keys(const Table& L, const Table& R, const std::vector<int>& left_keys, const std::vector<int>& right_keys) {
   FG_CHECK(!left_keys.empty() && left_keys.size() == right_keys.size(), FLOCKGPU_ERR_INVALID, "hash_join: key lists must be non-empty and of equal length");
   FG_CHECK(left_keys.size() <= size_t(MAX_KEY_COLS), FLOCKGPU_ERR_UNSUPPORTED, "hash_join: more than %d key columns", MAX_KEY_COLS);
   for (size_t i = 0; i < left_keys.size(); ++i) {
@@ -367,6 +436,51 @@ TablePtr hash_join(const CtxPtr& ctx, const TablePtr& left_ptr, const TablePtr& 
     FG_CHECK(lk >= 0 && lk < int(L.cols.size()) && rk >= 0 && rk < int(R.cols.size()), FLOCKGPU_ERR_INVALID, "hash_join: key column out of range");
     check_join_key_types("hash_join", L.cols[lk], R.cols[rk]);
   }
+}
+
+// kernel flavour: one fixed-width key column (KW = 4 / 8) or the general form (KW = 0)
+template <class F>
+static void by_width(int kw, F&& f) {
+  if (kw == 4) f(std::integral_constant<int, 4>{});
+  else if (kw == 8) f(std::integral_constant<int, 8>{});
+  else f(std::integral_constant<int, 0>{});
+}
+
+// The open-addressing table over the `bs.n_rows` rows of the build side, filled by join_build_kernel; *tbuf owns it.
+static JoinTable build_join_table(const CtxPtr& ctx, const JoinSide& bs, int kw, BufferPtr* tbuf) {
+  unsigned long long cap = 1024;
+  while (cap < 2ull * (unsigned long long)bs.n_rows) cap <<= 1;
+  JoinTable tab{};
+  if (kw == 4) {
+    // 16-byte slots (key, head, count), all-zero = empty, then next[build rows]
+    *tbuf = alloc(ctx, size_t(cap) * sizeof(JoinSlot) + size_t(bs.n_rows) * 4);
+    FG_CUDA(cudaMemsetAsync((*tbuf)->ptr, 0, size_t(cap) * sizeof(JoinSlot), ctx->stream));
+    tab.slots = (*tbuf)->as<JoinSlot>();
+    tab.next = reinterpret_cast<unsigned*>(tab.slots + cap);
+    tab.cap = cap;
+  } else {
+    // rep | head | cnt in one allocation (cap words each), then next[build rows]
+    *tbuf = alloc(ctx, size_t(cap) * 12 + size_t(bs.n_rows) * 4);
+    FG_CUDA(cudaMemsetAsync((*tbuf)->ptr, 0xff, size_t(cap) * 8, ctx->stream));                                  // rep, head = EMPTY
+    FG_CUDA(cudaMemsetAsync(static_cast<char*>((*tbuf)->ptr) + size_t(cap) * 8, 0, size_t(cap) * 4, ctx->stream));  // cnt = 0
+    unsigned* w = (*tbuf)->as<unsigned>();
+    tab = JoinTable{w, w + cap, w + 2 * cap, w + 3 * cap, cap, nullptr};
+  }
+  {
+    LaunchTimer lt(ctx, "join_build_kernel");
+    by_width(kw, [&](auto w) { join_build_kernel<decltype(w)::value><<<grid_for(ctx, bs.n_rows, 256, 8), 256, 0, ctx->stream>>>(bs, tab); });
+  }
+  FG_CUDA(cudaGetLastError());
+  count_launch(ctx);
+  return tab;
+}
+
+TablePtr hash_join(const CtxPtr& ctx, const TablePtr& left_ptr, const TablePtr& right_ptr, const std::vector<int>& left_keys,
+                   const std::vector<int>& right_keys) {
+  const Table& L = *left_ptr;
+  const Table& R = *right_ptr;
+  // the key columns are checked before any fast path, so every path accepts and refuses the same joins
+  check_join_keys(L, R, left_keys, right_keys);
   // one side is a single row and the other a group-by result still in table form (NEXMark q5: num = MAX(num)):
   // an equality selection over the table, no rows are materialised for the join
   if (left_keys.size() == 1 && right_keys.size() == 1) {
@@ -414,11 +528,6 @@ TablePtr hash_join(const CtxPtr& ctx, const TablePtr& left_ptr, const TablePtr& 
       bs.key0 = B.cols[(swap_sides ? right_keys : left_keys)[0]].values();
       ps.key0 = P.cols[(swap_sides ? left_keys : right_keys)[0]].values();
     }
-    auto by_width = [&](auto&& f) {
-      if (kw == 4) f(std::integral_constant<int, 4>{});
-      else if (kw == 8) f(std::integral_constant<int, 8>{});
-      else f(std::integral_constant<int, 0>{});
-    };
     if (kw && B.num_rows == 1 && bs.n_null_cols == 0 && ps.n_null_cols == 0 && ps.n_nan_cols == 0) {
       // one build row: equality filter over the probe side (see join_one_kernel), which compares bits only -- NULL and
       // NaN keys (a Float64 key column) take the table path, which skips them
@@ -429,7 +538,7 @@ TablePtr hash_join(const CtxPtr& ctx, const TablePtr& left_ptr, const TablePtr& 
       oa.n_rows = P.num_rows;
       oa.probe_idx = probe_idx->as<unsigned>();
       const int64_t num_tiles = (P.num_rows + CP_THREADS * 16 - 1) / (CP_THREADS * 16);
-      by_width([&](auto w) {
+      by_width(kw, [&](auto w) {
         constexpr int KW = decltype(w)::value == 8 ? 8 : 4;
         auto kernel = join_one_kernel<KW>;
         oa.sc = prepare_compact(ctx, num_tiles, resident_ctas(ctx, reinterpret_cast<const void*>(kernel), CP_THREADS), ctx->d_scalars + 4);
@@ -447,31 +556,8 @@ TablePtr hash_join(const CtxPtr& ctx, const TablePtr& left_ptr, const TablePtr& 
         FG_CUDA(cudaMemsetAsync(build_idx->ptr, 0, size_t(n_pairs) * 4, ctx->stream));
       }
     } else {
-    unsigned long long cap = 1024;
-    while (cap < 2ull * (unsigned long long)B.num_rows) cap <<= 1;
-    JoinTable tab{};
     BufferPtr tbuf;
-    if (kw == 4) {
-      // 16-byte slots (key, head, count), all-zero = empty, then next[build rows]
-      tbuf = alloc(ctx, size_t(cap) * sizeof(JoinSlot) + size_t(B.num_rows) * 4);
-      FG_CUDA(cudaMemsetAsync(tbuf->ptr, 0, size_t(cap) * sizeof(JoinSlot), ctx->stream));
-      tab.slots = tbuf->as<JoinSlot>();
-      tab.next = reinterpret_cast<unsigned*>(tab.slots + cap);
-      tab.cap = cap;
-    } else {
-      // rep | head | cnt in one allocation (cap words each), then next[build rows]
-      tbuf = alloc(ctx, size_t(cap) * 12 + size_t(B.num_rows) * 4);
-      FG_CUDA(cudaMemsetAsync(tbuf->ptr, 0xff, size_t(cap) * 8, ctx->stream));                                  // rep, head = EMPTY
-      FG_CUDA(cudaMemsetAsync(static_cast<char*>(tbuf->ptr) + size_t(cap) * 8, 0, size_t(cap) * 4, ctx->stream));  // cnt = 0
-      unsigned* w = tbuf->as<unsigned>();
-      tab = JoinTable{w, w + cap, w + 2 * cap, w + 3 * cap, cap, nullptr};
-    }
-    {
-      LaunchTimer lt(ctx, "join_build_kernel");
-      by_width([&](auto w) { join_build_kernel<decltype(w)::value><<<grid_for(ctx, B.num_rows, 256, 8), 256, 0, ctx->stream>>>(bs, tab); });
-    }
-    FG_CUDA(cudaGetLastError());
-    count_launch(ctx);
+    const JoinTable tab = build_join_table(ctx, bs, kw, &tbuf);
 
     BufferPtr off = alloc(ctx, size_t(P.num_rows + 1) * 4);
     JoinCountArgs ca{};
@@ -480,7 +566,7 @@ TablePtr hash_join(const CtxPtr& ctx, const TablePtr& left_ptr, const TablePtr& 
     ca.table = tab;
     ca.out_off = off->as<unsigned>();
     const int64_t num_tiles = (P.num_rows + JC_TILE - 1) / JC_TILE;
-    by_width([&](auto w) {
+    by_width(kw, [&](auto w) {
       auto kernel = join_count_scan_kernel<decltype(w)::value>;
       ca.sc = prepare_compact(ctx, num_tiles, resident_ctas(ctx, reinterpret_cast<const void*>(kernel), JC_THREADS), ctx->d_scalars + 4);
       LaunchTimer lt(ctx, "join_count_scan_kernel");
@@ -504,7 +590,7 @@ TablePtr hash_join(const CtxPtr& ctx, const TablePtr& left_ptr, const TablePtr& 
       ea.probe_idx = probe_idx->as<unsigned>();
       {
         LaunchTimer lt(ctx, "join_emit_kernel");
-        by_width([&](auto w) { join_emit_kernel<decltype(w)::value><<<grid_for(ctx, P.num_rows, 256, 8), 256, 0, ctx->stream>>>(ea); });
+        by_width(kw, [&](auto w) { join_emit_kernel<decltype(w)::value><<<grid_for(ctx, P.num_rows, 256, 8), 256, 0, ctx->stream>>>(ea); });
       }
       FG_CUDA(cudaGetLastError());
       count_launch(ctx);
@@ -526,6 +612,81 @@ TablePtr hash_join(const CtxPtr& ctx, const TablePtr& left_ptr, const TablePtr& 
   for (const Column& c : R.cols) rsrc.push_back(&c);
   for (Column& c : gather_columns(ctx, lsrc, l_idx, n_pairs)) out->cols.push_back(std::move(c));
   for (Column& c : gather_columns(ctx, rsrc, r_idx, n_pairs)) out->cols.push_back(std::move(c));
+  return out;
+}
+
+TablePtr hash_semi_join(const CtxPtr& ctx, const TablePtr& left_ptr, const TablePtr& right_ptr, const std::vector<int>& left_keys,
+                        const std::vector<int>& right_keys, bool anti) {
+  const Table& L = *left_ptr;
+  const Table& R = *right_ptr;
+  check_join_keys(L, R, left_keys, right_keys);
+  L.dense();
+  R.dense();
+  // a NULL key column (one-row global aggregate over empty input) matches nothing
+  bool null_key = false;
+  for (size_t i = 0; i < left_keys.size(); ++i) null_key |= L.cols[left_keys[i]].all_null || R.cols[right_keys[i]].all_null;
+  // the output is a subset of the left rows in their order: all of them is the left input itself, rows and routing
+  if (L.num_rows == 0) return left_ptr;
+  if (R.num_rows == 0 || null_key) return anti ? left_ptr : empty_like(ctx, L);
+
+  std::vector<int> widths;
+  for (int lk : left_keys) widths.push_back(L.cols[lk].width());
+  const bool packed = keys_packable(widths.data(), int(widths.size()));
+  const int kw = (packed && widths.size() == 1) ? widths[0] : 0;
+  JoinSide ls{}, rs{};
+  fill_side(L, left_keys, packed, &ls);
+  fill_side(R, right_keys, packed, &rs);
+  if (kw) {
+    ls.key0 = L.cols[left_keys[0]].values();
+    rs.key0 = R.cols[right_keys[0]].values();
+  }
+  // hash the smaller input, as the inner join does
+  const bool build_left = L.num_rows <= R.num_rows;
+  BufferPtr tbuf, marked;
+  const JoinTable tab = build_join_table(ctx, build_left ? ls : rs, kw, &tbuf);
+  if (build_left) {
+    marked = alloc(ctx, size_t(tab.cap));
+    FG_CUDA(cudaMemsetAsync(marked->ptr, 0, size_t(tab.cap), ctx->stream));
+    SemiMarkArgs ma{ls, rs, tab, marked->as<unsigned char>()};
+    {
+      LaunchTimer lt(ctx, "semi_mark_kernel");
+      by_width(kw, [&](auto w) { semi_mark_kernel<decltype(w)::value><<<grid_for(ctx, R.num_rows, 256, 8), 256, 0, ctx->stream>>>(ma); });
+    }
+    FG_CUDA(cudaGetLastError());
+    count_launch(ctx);
+  }
+  BufferPtr idx = alloc(ctx, size_t(L.num_rows) * 4);
+  SemiSelectArgs sa{};
+  sa.build = build_left ? ls : rs;
+  sa.left = ls;
+  sa.table = tab;
+  sa.marked = build_left ? marked->as<unsigned char>() : nullptr;
+  sa.keep_matched = anti ? 0 : 1;
+  sa.out_idx = idx->as<unsigned>();
+  const int64_t num_tiles = (L.num_rows + CP_THREADS * 16 - 1) / (CP_THREADS * 16);
+  by_width(kw, [&](auto w) {
+    auto kernel = semi_select_kernel<decltype(w)::value>;
+    sa.sc = prepare_compact(ctx, num_tiles, resident_ctas(ctx, reinterpret_cast<const void*>(kernel), CP_THREADS), ctx->d_scalars + 4);
+    LaunchTimer lt(ctx, "semi_select_kernel");
+    launch_compact(ctx, kernel, sa.sc, sa);
+  });
+  FG_CUDA(cudaGetLastError());
+  count_launch(ctx);
+  unsigned long long total = 0;
+  read_scalars(ctx, 4, 1, &total);
+  FG_CHECK(total <= (unsigned long long)L.num_rows, FLOCKGPU_ERR_CUDA, "hash_join: corrupt semi / anti row count");
+  if (total == (unsigned long long)L.num_rows) return left_ptr;
+  if (total == 0) return empty_like(ctx, L);
+  auto out = std::make_shared<Table>();
+  out->ctx = ctx;
+  out->metadata = L.metadata;
+  out->num_rows = int64_t(total);
+  // the kept rows stay on the rank they were routed to
+  out->partitioned_on = L.partitioned_on;
+  out->partition_world = L.partition_world;
+  std::vector<const Column*> src;
+  for (const Column& c : L.cols) src.push_back(&c);
+  out->cols = gather_columns(ctx, src, idx->as<uint32_t>(), out->num_rows);
   return out;
 }
 

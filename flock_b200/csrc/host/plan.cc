@@ -707,7 +707,7 @@ static JoinCount join_count(const ExecEnv& env, const HashAggregateExec& agg, co
   for (const auto& g : agg.group_expr)
     if (!is_column_expr(*g.first)) return {};
   auto* join = dynamic_cast<HashJoinExec*>(skip_to_operator(agg.input.get()));
-  if (!join || join->on.size() != 1) return {};
+  if (!join || join->join_type != HashJoinExec::Type::Inner || join->on.size() != 1) return {};
   // a FilterExec below a join input (through pass-throughs) hands over its input: its predicate may move into the kernel
   TablePtr in[2];
   FilterExec* filter[2] = {};
@@ -861,7 +861,8 @@ TablePtr HashAggregateExec::execute_uncached(const ExecEnv& env) {
 }
 
 std::string HashJoinExec::fmt_as() const {
-  std::string s = "HashJoinExec: mode=" + mode + ", join_type=Inner, on=[";
+  const char* type = join_type == Type::Semi ? "Semi" : join_type == Type::Anti ? "Anti" : "Inner";
+  std::string s = "HashJoinExec: mode=" + mode + ", join_type=" + type + ", on=[";
   for (size_t i = 0; i < on.size(); ++i) s += std::string(i ? ", " : "") + "(" + on[i].first.name + ", " + on[i].second.name + ")";
   return s + "]";
 }
@@ -874,6 +875,7 @@ TablePtr HashJoinExec::join(const ExecEnv& env, const TablePtr& l, const TablePt
     lk.push_back(resolve_column(*l, p.first.name, p.first.index));
     rk.push_back(resolve_column(*r, p.second.name, p.second.index));
   }
+  if (join_type != Type::Inner) return fg::hash_semi_join(env.ctx, l, r, lk, rk, join_type == Type::Anti);
   return fg::hash_join(env.ctx, l, r, lk, rk);
 }
 
@@ -1028,7 +1030,9 @@ static PlanPtr build_plan(const Json& j) {
   if (tag == "hash_join_exec") {
     auto n = std::make_shared<HashJoinExec>();
     const std::string& jt = j.at("join_type").as_string("join_type");
-    if (jt != "Inner") fail(FLOCKGPU_ERR_UNSUPPORTED, "plan: join_type %s is not supported on the GPU path (Inner only)", jt.c_str());
+    if (jt == "Semi") n->join_type = HashJoinExec::Type::Semi;
+    else if (jt == "Anti") n->join_type = HashJoinExec::Type::Anti;
+    else if (jt != "Inner") fail(FLOCKGPU_ERR_UNSUPPORTED, "plan: join_type %s is not supported on the GPU path (Inner, Semi and Anti only)", jt.c_str());
     if (const Json* m = j.get("mode")) n->mode = m->is_string() ? m->str : "Partitioned";
     for (const JsonPtr& pair : j.at("on").arr) {
       if (!pair->is_array() || pair->arr.size() != 2) fail(FLOCKGPU_ERR_INVALID, "plan JSON: join `on` entries must be pairs");

@@ -149,6 +149,8 @@ class HashJoinExec : public ExecutionPlan {
   };
   std::vector<std::pair<OnCol, OnCol>> on;
   std::string mode = "Partitioned";
+  // Semi / Anti output the left input's columns only: the left rows with (without) an equal key on the right
+  enum class Type { Inner, Semi, Anti } join_type = Type::Inner;
   const char* name() const override { return "HashJoinExec"; }
   std::vector<PlanPtr> children() const override { return {left, right}; }
   std::string fmt_as() const override;

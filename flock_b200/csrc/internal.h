@@ -550,6 +550,11 @@ TablePtr hash_aggregate(const CtxPtr& ctx, const TablePtr& in, int mode, const s
 double distinct_sample_duplicates(const CtxPtr& ctx, const TablePtr& in, const std::vector<int>& group_cols);
 TablePtr hash_join(const CtxPtr& ctx, const TablePtr& left, const TablePtr& right,
                    const std::vector<int>& left_keys, const std::vector<int>& right_keys);
+// HashJoinExec { join_type: Semi } (anti = false) / { Anti } (anti = true): the rows of `left` whose key tuple occurs
+// (does not occur) in `right`, each at most once, in left order, with the left schema.  Key equality and the key type
+// checks are hash_join's: a NULL or NaN component matches nothing.
+TablePtr hash_semi_join(const CtxPtr& ctx, const TablePtr& left, const TablePtr& right,
+                        const std::vector<int>& left_keys, const std::vector<int>& right_keys, bool anti);
 // COUNT(*) of `fact JOIN dim ON fact.fact_key = dim.dim_key` (inner) [WHERE `predicate` over the fact's columns],
 // grouped by the dimension's `group_cols`, in one pass over the fact (dim_count.cu).  Output: the group columns under
 // their dimension names, then one UInt64 count column per name of `count_names` (COUNT(*) listed n times: n equal

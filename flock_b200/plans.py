@@ -129,8 +129,10 @@ def hash_aggregate_exec(mode: str, group_expr: list[tuple[dict, str]], aggr_expr
             "aggr_expr": aggr_expr, "input": input}
 
 
-def hash_join_exec(left: dict, right: dict, on: list[tuple[dict, dict]], mode: str = "Partitioned") -> dict:
-    return {"execution_plan": "hash_join_exec", "join_type": "Inner", "mode": mode, "left": left, "right": right,
+def hash_join_exec(left: dict, right: dict, on: list[tuple[dict, dict]], mode: str = "Partitioned", join_type: str = "Inner") -> dict:
+    """join_type "Inner": left ++ right columns; "Semi" / "Anti": the left rows with / without an equal key on the right,
+    left columns only (DataFusion 6's JoinType variant names)."""
+    return {"execution_plan": "hash_join_exec", "join_type": join_type, "mode": mode, "left": left, "right": right,
             "on": [[{"name": l["name"], "index": l["index"]}, {"name": r["name"], "index": r["index"]}] for l, r in on]}
 
 
@@ -713,3 +715,107 @@ TPCH_MORE_QUERIES = {"q7": tpch_q7, "q8": tpch_q8, "q9": tpch_q9}
 TPCH_MORE_SOURCES = {"q7": ["supplier", "lineitem", "orders", "customer", "nation", "nation"],
                      "q8": ["supplier", "lineitem", "part", "orders", "customer", "nation", "nation", "region"],
                      "q9": ["supplier", "lineitem", "part", "partsupp", "orders", "nation"]}
+
+
+# ---- TPC-H q4, q16, q18 and q21: EXISTS, IN and NOT IN subqueries as Semi / Anti hash joins ----------------------------------
+# Shape unverified, like the queries above.  A subquery becomes the right input of a Partitioned Semi (EXISTS, IN) or Anti
+# (NOT EXISTS, NOT IN) join on its correlation key; the join keeps the left input's columns.  q21's correlated
+# conditions have no key equality (l2.l_suppkey <> l1.l_suppkey), and DataFusion 6's HashJoinExec has no join filter,
+# so they are decorrelated into per-order counts: another supplier on the order exists iff the order has at least two
+# distinct suppliers, and no other late supplier exists iff the order's one late supplier is l1's own (l1 is late).
+# COUNT(DISTINCT x) is DataFusion's single-distinct rewrite: group by (keys, x), then COUNT(*) grouped by the keys.
+def _semi(left: _Rel, right: _Rel, on: list[tuple[str, str]], n: int, join_type: str = "Semi", as_inner: bool = False) -> _Rel:
+    """left Semi / Anti right.  `as_inner` plans a Semi join the way it is written without one, for comparison:
+    DISTINCT over the right keys, then an inner join (left ++ the right keys)."""
+    if as_inner:
+        assert join_type == "Semi"
+        keys = _grouped(right, [b for _, b in on], [], n)
+        return _join(left, keys, on, n)
+    lsh = coalesce_batches_exec(repartition_hash(left.plan, [left.c(a) for a, _ in on], n))
+    rsh = coalesce_batches_exec(repartition_hash(right.plan, [right.c(b) for _, b in on], n))
+    return _Rel(coalesce_batches_exec(hash_join_exec(lsh, rsh, [(left.c(a), right.c(b)) for a, b in on], join_type=join_type)), left.names)
+
+
+def _count(name: str) -> dict:
+    return aggregate_expr("count", name, literal("UInt8", 1), "UInt64")
+
+
+def tpch_q4(n: int = TARGET_PARTITIONS, as_inner: bool = False) -> dict:
+    # DATE '1993-07-01' + interval '3' month, folded
+    od = _filter(_tpch_scan("orders", ["o_orderkey", "o_orderdate", "o_orderpriority"], n),
+                 lambda r: _and(binary(r.c("o_orderdate"), "GtEq", _date("1993-07-01")), binary(r.c("o_orderdate"), "Lt", _date("1993-10-01"))))
+    li = _filter(_tpch_scan("lineitem", ["l_orderkey", "l_commitdate", "l_receiptdate"], n),
+                 lambda r: binary(r.c("l_commitdate"), "Lt", r.c("l_receiptdate")))
+    j = _semi(od, li, [("o_orderkey", "l_orderkey")], n, as_inner=as_inner)
+    cnt = _count("COUNT(UInt8(1))")
+    g = _grouped(j, ["o_orderpriority"], [cnt], n)
+    return _project_sort(g, [(g.c("o_orderpriority"), "o_orderpriority"), (g.c(cnt["name"]), "order_count")], [("o_orderpriority", False)])
+
+
+def tpch_q16(n: int = TARGET_PARTITIONS, anti: bool = True) -> dict:
+    """`anti=False` leaves out the NOT IN (supplier complaints) join."""
+    ps = _tpch_scan("partsupp", ["ps_partkey", "ps_suppkey"], n)
+    sizes = [literal("Int32", s) for s in (49, 14, 23, 45, 19, 3, 36, 9)]
+    pt = _filter(_tpch_scan("part", ["p_partkey", "p_brand", "p_type", "p_size"], n),
+                 lambda r: _and(binary(r.c("p_brand"), "NotEq", literal("Utf8", "Brand#45")),
+                                binary(r.c("p_type"), "NotLike", literal("Utf8", "MEDIUM POLISHED%")), in_list(r.c("p_size"), sizes)))
+    j = _join(ps, pt, [("ps_partkey", "p_partkey")], n)
+    if anti:
+        su = _filter(_tpch_scan("supplier", ["s_suppkey", "s_comment"], n),
+                     lambda r: binary(r.c("s_comment"), "Like", literal("Utf8", "%Customer%Complaints%")))
+        j = _semi(j, su, [("ps_suppkey", "s_suppkey")], n, "Anti")
+    pairs = _grouped(j, ["p_brand", "p_type", "p_size", "ps_suppkey"], [], n)
+    cnt = _count("COUNT(DISTINCT partsupp.ps_suppkey)")
+    g = _grouped(pairs, ["p_brand", "p_type", "p_size"], [cnt], n)
+    return _project_sort(g, [(g.c("p_brand"), "p_brand"), (g.c("p_type"), "p_type"), (g.c("p_size"), "p_size"), (g.c(cnt["name"]), "supplier_cnt")],
+                         [("supplier_cnt", True), ("p_brand", False), ("p_type", False), ("p_size", False)])
+
+
+def tpch_q18(n: int = TARGET_PARTITIONS, as_inner: bool = False) -> dict:
+    qty = _sum("SUM(lineitem.l_quantity)", column("l_quantity", 1))
+    big = _grouped(_tpch_scan("lineitem", ["l_orderkey", "l_quantity"], n), ["l_orderkey"], [qty], n)
+    big = _filter(big, lambda r: binary(r.c(qty["name"]), "Gt", _f64(300)))
+    cu = _tpch_scan("customer", ["c_custkey", "c_name"], n)
+    od = _tpch_scan("orders", ["o_orderkey", "o_custkey", "o_totalprice", "o_orderdate"], n)
+    li = _tpch_scan("lineitem", ["l_orderkey", "l_quantity"], n)
+    od = _semi(od, big, [("o_orderkey", "l_orderkey")], n, as_inner=as_inner)
+    if as_inner:  # drop the DISTINCT keys: the joins below name l_orderkey / l_quantity of the second lineitem scan
+        od = _subquery(od, [(od.c(c), c) for c in ("o_orderkey", "o_custkey", "o_totalprice", "o_orderdate")])
+    j = _join(cu, od, [("c_custkey", "o_custkey")], n)
+    j = _join(j, li, [("o_orderkey", "l_orderkey")], n)
+    total = _sum("SUM(lineitem.l_quantity)", j.c("l_quantity"))
+    g = _grouped(j, ["c_name", "c_custkey", "o_orderkey", "o_orderdate", "o_totalprice"], [total], n)
+    return _project_sort(g, [(g.c(c), c) for c in ("c_name", "c_custkey", "o_orderkey", "o_orderdate", "o_totalprice")] +
+                         [(g.c(total["name"]), "SUM(lineitem.l_quantity)")], [("o_totalprice", True), ("o_orderdate", False)])
+
+
+def _orders_with_suppliers(li: _Rel, name: str, n: int) -> _Rel:
+    """The l_orderkey of orders with more than one distinct l_suppkey among the lines of `li`."""
+    pairs = _grouped(li, ["l_orderkey", "l_suppkey"], [], n)
+    g = _grouped(pairs, ["l_orderkey"], [_count(name)], n)
+    return _filter(g, lambda r: binary(r.c(name), "Gt", literal("UInt64", 1)))
+
+
+def tpch_q21(n: int = TARGET_PARTITIONS) -> dict:
+    late = lambda r: binary(r.c("l_receiptdate"), "Gt", r.c("l_commitdate"))
+    su = _tpch_scan("supplier", ["s_suppkey", "s_name", "s_nationkey"], n)
+    l1 = _filter(_tpch_scan("lineitem", ["l_orderkey", "l_suppkey", "l_commitdate", "l_receiptdate"], n), late)
+    l2 = _tpch_scan("lineitem", ["l_orderkey", "l_suppkey"], n)
+    l3 = _filter(_tpch_scan("lineitem", ["l_orderkey", "l_suppkey", "l_commitdate", "l_receiptdate"], n), late)
+    od = _filter(_tpch_scan("orders", ["o_orderkey", "o_orderstatus"], n), lambda r: binary(r.c("o_orderstatus"), "Eq", literal("Utf8", "F")))
+    na = _filter(_tpch_scan("nation", ["n_nationkey", "n_name"], n), lambda r: binary(r.c("n_name"), "Eq", literal("Utf8", "SAUDI ARABIA")))
+    l1 = _semi(l1, _orders_with_suppliers(l2, "COUNT(DISTINCT l2.l_suppkey)", n), [("l_orderkey", "l_orderkey")], n, "Semi")
+    l1 = _semi(l1, _orders_with_suppliers(l3, "COUNT(DISTINCT l3.l_suppkey)", n), [("l_orderkey", "l_orderkey")], n, "Anti")
+    j = _join(su, l1, [("s_suppkey", "l_suppkey")], n)
+    j = _join(j, od, [("l_orderkey", "o_orderkey")], n)
+    j = _join(j, na, [("s_nationkey", "n_nationkey")], n)
+    cnt = _count("COUNT(UInt8(1))")
+    g = _grouped(j, ["s_name"], [cnt], n)
+    return _project_sort(g, [(g.c("s_name"), "s_name"), (g.c(cnt["name"]), "numwait")], [("numwait", True), ("s_name", False)])
+
+
+# Kept apart from TPCH_QUERIES and TPCH_MORE_QUERIES, whose entries the existing suites and tools iterate.
+TPCH_SUBQUERY_QUERIES = {"q4": tpch_q4, "q16": tpch_q16, "q18": tpch_q18, "q21": tpch_q21}
+TPCH_SUBQUERY_SOURCES = {"q4": ["orders", "lineitem"], "q16": ["partsupp", "part", "supplier"],
+                         "q18": ["lineitem", "customer", "orders", "lineitem"],
+                         "q21": ["supplier", "lineitem", "lineitem", "lineitem", "orders", "nation"]}

@@ -347,7 +347,9 @@ int flockgpu_hash_aggregate(flockgpu_ctx* ctx, const flockgpu_table* in, int32_t
 /* ---- HashJoinExec { mode: Partitioned, join_type: Inner } (planner.rs:169, :239) ---------------
  * out = left ++ right columns for every pair with equal keys (NULL != NULL; duplicates give the
  * full cross product).  `left` is the build side, exactly as in the reference (the textual left of
- * the SQL join).  Key column types must match pairwise (Int32/Int64/UInt64/Timestamp/Utf8).        */
+ * the SQL join).  Key column types must match pairwise (Int32/Int64/UInt64/Timestamp/Utf8).
+ * join_type Semi / Anti (the left rows with / without an equal key on the right) is reached
+ * through plans (flock_context_unmarshal), not through this call.                                  */
 int flockgpu_hash_join(flockgpu_ctx* ctx, const flockgpu_table* left, const flockgpu_table* right,
                        const int32_t* left_keys, const int32_t* right_keys, int32_t n_keys,
                        flockgpu_table** out);
